@@ -3,7 +3,7 @@
 
 Metric (BASELINE.json): DAS channels/s through the f-k filter (+ matched filter), plus achieved HBM GB/s vs the
 measured roofline.  Workload at N=1: BASELINE.json configs[1] -- synthetic 10 000 ch x 120 000 samp fp32, f-k filter
-only (dsp.fk_filter_design fan mask), 1 x B200.  At N>1 every rank filters its own 10 000 x 120 000 file (files are
+only (dsp.fk_filter_design fan mask), 1 x H100.  At N>1 every rank filters its own 10 000 x 120 000 file (files are
 independent: weak scaling, no data-path collective); additionally, at N>1, one 20 000 x 240 000 matrix is filtered
 channel-sharded over all ranks with NCCL all-to-all transposes (BASELINE configs[3]) and reported under `sharded_fk`.
 
@@ -14,7 +14,11 @@ Extra legs in the same JSON line (all device-timed with CUDA events unless state
   pipeline_e2e              BASELINE configs[4]'s per-GPU work: pipeline.MfDetectPipeline, int32 counts up, picks down
   cpu_baseline              the oracle port of the reference path on the box's host cores (N=1 only)
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
+
+--dump-outputs DIR writes what the last timed step returned to its caller as DIR/*.npy: a fixed, seeded sample of
+DUMP_ROWS channels of the filtered matrix (float32, full time axis) and their channel indices (float64).  The input
+matrix is generated from a fixed seed, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -36,14 +40,11 @@ ALGO_BYTES_PER_SAMPLE = 24          # SURVEY.md 8(d): 3 HBM round trips x (read 
 MF_BYTES_PER_SAMPLE = 12            # SURVEY.md 8(d): matched filter, 2 templates: read 4 + write 8
 METRIC = "DAS channels/sec through f-k filter"
 WORKLOAD = f"synthetic {NX} ch x {NS} samp fp32, f-k filter only (fk_filter_design fan mask {FAN}), one matrix per GPU"
-CONFIG = {"workload": WORKLOAD, "l2": "inputs (4.8 GB) exceed the 126 MB L2; no flush needed"}   # identical in both arms
+CONFIG = {"workload": WORKLOAD, "l2": "inputs (4.8 GB) exceed the 50 MB L2; no flush needed"}   # identical in both arms
 CPU_SAMPLE_NX = 250                 # single-thread sample: 250 channels x the full 120 000 samples
 SHARD_NX, SHARD_NS = 20000, 240000  # BASELINE configs[3]
 
-# ncu --set full dram__bytes_read.sum + dram__bytes_write.sum per launch, keyed by what was profiled: (column scheme,
-# kept rows).  Used only when the plan that runs equals the profiled one; otherwise `traffic` is null.
-NCU_TRAFFIC = {(3, 1356): {"step": 7.390e9 + 2.547e9 + 3.256e9 + 2.546e9 + 8.044e9, "p5": 8.044e9,
-                           "src": "profiles/r02_fk_pipe.txt (P1 7.390, P2 2.547, P3 3.256, P4 2.546, P5 8.044 GB)"}}
+DUMP_ROWS, DUMP_SEED = 64, 0        # --dump-outputs: 64 x 120 000 float32 = 31 MB
 COL_KERNEL = {0: "k_col_inv_dual", 1: "k_col_inv_tma", 2: "k_colB_inv_fused + k_colA_inv", 3: "k_col2_pipe<inverse>"}
 
 
@@ -52,7 +53,7 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s, not a measured figure)"
 
 
 def mem_available_gb():
@@ -240,6 +241,7 @@ def main():
     ap.add_argument("--no-hybrid", action="store_true")
     ap.add_argument("--no-pipeline", action="store_true")
     ap.add_argument("--no-sharded", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's output sample as DIR/*.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -323,6 +325,11 @@ def main():
     e1.record()
     barrier()
     launches = L.d4w_launch_count() - n0
+    if args.dump_outputs and rank == 0:
+        rows = np.sort(np.random.default_rng(DUMP_SEED).choice(NX, DUMP_ROWS, replace=False))
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "fk_filtered_rows.npy"), y[torch.from_numpy(rows).to(y.device)].cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "fk_filtered_rows_channels.npy"), rows.astype(np.float64))
     clocks = None
     if rank == 0:
         # nvidia-smi reports every 100 ms; a short timed region (K steps of ~8 ms) may see fewer than three reports, so
@@ -553,7 +560,7 @@ def main():
                        "serial_schedule": {"ms_per_step": serial_ms, "stage_ms_rank0": stage_ms, "all_to_all_ms": round(a2a_ms, 3),
                                            "compute_and_permute_ms": round(sum(stage_ms.values()) - a2a_ms, 3),
                                            "nvlink_gbs_per_rank_during_exchanges": round((2 * real_b + 2 * spec_b) / max(a2a_ms, 1e-6) / 1e6, 1)},
-                       "note": "SURVEY 8(d) bound for 4 GPUs: 2 x 3.6 GB per GPU per direction at 900 GB/s = 8 ms of pure exchange"}
+                       "note": "SURVEY 8(d) bound for 4 GPUs: 2 x 3.6 GB per GPU per direction at 450 GB/s (H100 NVLink 4) = 16 ms of pure exchange"}
             del sflt, be, xl, smask
         except Exception as exc:            # noqa: BLE001
             sharded = {"unavailable": repr(exc)[:300]}
@@ -564,7 +571,6 @@ def main():
         achieved = algo_bytes / (ms_step * 1e-3) / 1e9
         traffic = flt.traffic_bytes()
         scheme = flt.plan.col_scheme
-        prof = NCU_TRAFFIC.get((scheme, flt.rows_kept))
         kernels = {n: {"ms": round(pass_ms[i], 4), "actual_bytes": traffic[n],
                        "actual_gbs": round(traffic[n] / (pass_ms[i] * 1e-3) / 1e9, 1) if pass_ms[i] > 0 else None}
                    for i, n in enumerate(names)}
@@ -572,7 +578,7 @@ def main():
         dom_alg = 8 * NX * NS          # SURVEY 8(d) K3: 4 B read + 4 B written per (channel, sample)
         dom = {"name": COL_KERNEL.get(scheme, "?") + " (P5, C2R over channels)", "ms": round(dom_ms, 4), "algorithmic_bytes": dom_alg,
                "achieved": round(dom_alg / (dom_ms * 1e-3) / 1e9, 1), "frac": round(dom_alg / (dom_ms * 1e-3) / 1e9 / peak, 4),
-               "traffic": prof["p5"] if prof else None}
+               "traffic": None}
         line = {"metric": METRIC, "value": value, "unit": "channels/s", "n_gpus": world, "steps": steps, "warmup": warmup,
                 "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                 "dtype": "f32", "data": "synthetic", "config": dict(CONFIG),
@@ -580,10 +586,9 @@ def main():
                          "col_tile_samples": flt.plan.tile, "col_scheme": scheme, "plan_bytes_per_step": sum(traffic.values())},
                 "gpu_launches": int(launches),
                 "roofline": {"bound": "hbm", "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s",
-                             "frac": round(achieved / peak, 4), "traffic": prof["step"] if prof else None,
-                             "traffic_source": ("ncu --set full dram__bytes_read+write per launch, " + prof["src"]) if prof else
-                                               "no ncu capture of this exact plan (scheme, kept rows): see plan.plan_bytes_per_step "
-                                               "for the bytes the plan must move",
+                             "frac": round(achieved / peak, 4), "traffic": None,
+                             "traffic_source": "no DRAM byte-counter capture: see plan.plan_bytes_per_step for the bytes the plan "
+                                               "must move",
                              "dominant_kernel": dom, "peak_source": peak_src,
                              "scope": "whole f-k filter = 5 kernels per step; achieved = 24 B/(channel*sample) algorithmic bytes "
                                       "(SURVEY 8d) / step time; actual_bytes per kernel below are lower because wavenumber rows "

@@ -1,4 +1,4 @@
-"""das4whales_b200 -- B200-native (sm_100a) implementation of the DAS4Whales channel-parallel
+"""das4whales_b200 -- H100-native (sm_90a) implementation of the DAS4Whales channel-parallel
 DSP hot path: f-k filter, band-pass, spectrogram, matched-filter / spectrogram correlators.
 
     import das4whales_b200 as dw

@@ -1,7 +1,7 @@
-"""Build libd4w.so (all CUDA kernels + the C ABI) for sm_100a, in-tree, with nvcc.
+"""Build libd4w.so (all CUDA kernels + the C ABI) for the H100 (sm_90a), in-tree, with nvcc.
 
-`nvcc` cross-compiles without a GPU, so this runs in the CPU-only build container; the
-resulting das4whales_b200/libd4w.so travels to the GPU box with the source snapshot.
+`nvcc` cross-compiles without a GPU, so the library can be built on a machine without one and
+copied with the source tree to the GPU machine.
 """
 import os
 import shutil
@@ -11,7 +11,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libd4w.so")
 SOURCES = ["d4w_fk.cu", "d4w_rows.cu", "d4w_image.cu"]
-NVCC_FLAGS = ["-std=c++17", "-O3", "--expt-relaxed-constexpr", "-gencode", "arch=compute_100a,code=sm_100a",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ["-std=c++17", "-O3", "--expt-relaxed-constexpr"] + GENCODE + [
               "-lineinfo", "-Xcompiler", "-fPIC", "-Wno-deprecated-gpu-targets"]
 
 
@@ -26,7 +27,8 @@ def _stale():
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "d4w.h")]
+    # this file too: a library built with other flags (another architecture) is stale
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "d4w.h"), __file__]
     return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))
 
 
@@ -60,7 +62,7 @@ def build_library(force=False, verbose=False):
             print(out)
         if p.returncode != 0:
             raise RuntimeError("nvcc failed: " + " ".join(cmd) + "\n" + (out or ""))
-    cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs + ["-lcudart"]
+    cmd = [_nvcc(), "-shared"] + GENCODE + ["-o", LIB] + objs + ["-lcudart"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed: " + " ".join(cmd) + "\n" + r.stdout)

@@ -64,7 +64,7 @@ static bool make_tile_map(CUtensorMap* map, const float* base, int nx, int ns) {
 
 struct d4w_fk_plan {
     int nx = 0, ns = 0, device = 0;
-    int num_sms = 148;
+    int num_sms = 0;                          // cudaDeviceProp::multiProcessorCount
     int t1 = 1, t2 = 0;
     ColParams col{};
     RowParams row{};

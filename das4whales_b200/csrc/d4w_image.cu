@@ -7,9 +7,15 @@
 
 using namespace d4w;
 
-static inline unsigned grid1d(size_t n, int threads, unsigned cap = 148 * 16) {
+// grid-stride kernels: at most `per_sm` CTAs per SM of the current device
+static inline unsigned grid1d(size_t n, int threads, unsigned per_sm = 16) {
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1) {
+        (void)cudaGetLastError();
+        sms = 1;
+    }
     const size_t b = (n + threads - 1) / threads;
-    return (unsigned)std::max<size_t>(1, std::min<size_t>(b, cap));
+    return (unsigned)std::max<size_t>(1, std::min<size_t>(b, (size_t)sms * per_sm));
 }
 
 extern "C" int d4w_scale_pixels(const float* x, float* y, size_t n, float mul, void* dev_ws8, void* stream_v) {
@@ -20,7 +26,7 @@ extern "C" int d4w_scale_pixels(const float* x, float* y, size_t n, float mul, v
     D4W_CHECK_LAUNCH("k_minmax_init");
     k_minmax<<<grid1d(n, 256), 256, 0, stream>>>(x, n, mm);
     D4W_CHECK_LAUNCH("k_minmax");
-    k_scale_pixels<<<grid1d(n, 256, 148 * 32), 256, 0, stream>>>(x, y, n, mm, mul);
+    k_scale_pixels<<<grid1d(n, 256, 32), 256, 0, stream>>>(x, y, n, mm, mul);
     D4W_CHECK_LAUNCH("k_scale_pixels");
     return D4W_OK;
 }
@@ -33,7 +39,7 @@ extern "C" int d4w_db_re_max(const float* x, float* y, size_t n, void* dev_ws8, 
     D4W_CHECK_LAUNCH("k_minmax_init");
     k_minmax<<<grid1d(n, 256), 256, 0, stream>>>(x, n, mm);
     D4W_CHECK_LAUNCH("k_minmax");
-    k_db_re_max<<<grid1d(n, 256, 148 * 32), 256, 0, stream>>>(x, y, n, mm);
+    k_db_re_max<<<grid1d(n, 256, 32), 256, 0, stream>>>(x, y, n, mm);
     D4W_CHECK_LAUNCH("k_db_re_max");
     return D4W_OK;
 }

@@ -1,35 +1,31 @@
-// fft_dual.cuh -- two-lane ("dual column") variant of the FFT engine built on Blackwell's
-// packed fp32x2 arithmetic (PTX fma/add/sub/mul .f32x2 -> SASS FFMA2 / FADD2 / FMUL2).
+// fft_dual.cuh -- two-lane ("dual column") variant of the FFT engine.
 //
 // The column passes of the f-k filter transform a tile of 4 consecutive time samples per
 // channel = two complex columns that undergo IDENTICAL butterflies with IDENTICAL twiddles.
 // Element c of the tile is stored as 16 bytes {reA, reB, imA, imB}; one thread runs both
-// columns through one instruction stream: every complex add/mul/fma is one packed instruction,
-// twiddles (per-lane equal) enter as broadcast scalar operands, shared memory traffic is
-// LDS.128 / STS.128 and the global side is one 16-byte cp.async per channel row.
-// Same __host__ __device__ discipline as fft_smem.cuh: on the host a lane pair is two floats.
+// columns through one instruction stream: the twiddles (per-lane equal) are loaded and formed
+// once for both lanes, shared memory traffic is LDS.128 / STS.128 and the global side is one
+// 16-byte cp.async per channel row.  Hopper has no packed fp32x2 arithmetic, so every lane op
+// is one scalar FADD / FMUL / FFMA; the _rn intrinsics stop nvcc from contracting a vmul that
+// feeds a vadd into an FFMA, so each lane rounds exactly as the operation written.
+// Same __host__ __device__ discipline as fft_smem.cuh.
 #pragma once
 #include "fft_smem.cuh"
 
 namespace d4w {
 
-// ---------------------------------------------------------------- packed pair of floats
+// ---------------------------------------------------------------- pair of floats
+struct __align__(8) f2x { float a, b; };
+D4W_HD f2x f2x_set(float a, float b) { f2x r; r.a = a; r.b = b; return r; }
+D4W_HD f2x vbc(float s) { return f2x_set(s, s); }
+D4W_HD float f2x_lo(f2x v) { return v.a; }
+D4W_HD float f2x_hi(f2x v) { return v.b; }
 #ifdef __CUDA_ARCH__
-struct f2x { unsigned long long v; };
-__device__ __forceinline__ f2x f2x_set(float a, float b) { f2x r; asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ f2x vbc(float s) { return f2x_set(s, s); }
-__device__ __forceinline__ float f2x_lo(f2x a) { return __uint_as_float((unsigned)(a.v & 0xffffffffull)); }
-__device__ __forceinline__ float f2x_hi(f2x a) { return __uint_as_float((unsigned)(a.v >> 32)); }
-__device__ __forceinline__ f2x vadd(f2x a, f2x b) { f2x r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v)); return r; }
-__device__ __forceinline__ f2x vsub(f2x a, f2x b) { f2x r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v)); return r; }
-__device__ __forceinline__ f2x vmul(f2x a, f2x b) { f2x r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v)); return r; }
-__device__ __forceinline__ f2x vfma(f2x a, f2x b, f2x c) { f2x r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r.v) : "l"(a.v), "l"(b.v), "l"(c.v)); return r; }
+__device__ __forceinline__ f2x vadd(f2x a, f2x b) { return f2x_set(__fadd_rn(a.a, b.a), __fadd_rn(a.b, b.b)); }
+__device__ __forceinline__ f2x vsub(f2x a, f2x b) { return f2x_set(__fsub_rn(a.a, b.a), __fsub_rn(a.b, b.b)); }
+__device__ __forceinline__ f2x vmul(f2x a, f2x b) { return f2x_set(__fmul_rn(a.a, b.a), __fmul_rn(a.b, b.b)); }
+__device__ __forceinline__ f2x vfma(f2x a, f2x b, f2x c) { return f2x_set(__fmaf_rn(a.a, b.a, c.a), __fmaf_rn(a.b, b.b, c.b)); }
 #else
-struct f2x { float a, b; };
-inline f2x f2x_set(float a, float b) { f2x r; r.a = a; r.b = b; return r; }
-inline f2x vbc(float s) { return f2x_set(s, s); }
-inline float f2x_lo(f2x v) { return v.a; }
-inline float f2x_hi(f2x v) { return v.b; }
 inline f2x vadd(f2x a, f2x b) { return f2x_set(a.a + b.a, a.b + b.b); }
 inline f2x vsub(f2x a, f2x b) { return f2x_set(a.a - b.a, a.b - b.b); }
 inline f2x vmul(f2x a, f2x b) { return f2x_set(a.a * b.a, a.b * b.b); }

@@ -1,4 +1,4 @@
-// fft_radix.cuh -- in-register radix-R DFT butterflies for the sm_100a FFT engine.
+// fft_radix.cuh -- in-register radix-R DFT butterflies for the sm_90a FFT engine.
 //
 // Every butterfly is a fully unrolled template: operands live in registers, twiddles
 // W_R^j are compile-time constants (constexpr-evaluated in double, rounded once to fp32),

@@ -60,7 +60,9 @@ inline const std::vector<int>& split_radices() {
 }
 
 // returns 0 on success; 1 = unsupported shape (err says why)
-inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, std::string& err, bool allow_row_dual = true) {
+// row_fused_default: whether the middle row pass uses k_row_mid_fused unless D4W_ROW_FUSED says otherwise
+inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, std::string& err, bool allow_row_dual = true,
+                             int row_fused_default = 0) {
     hp.nx = nx; hp.ns = ns;
     const int col_maxr = env_int("D4W_COL_MAX_RADIX", 25);
     const int row_maxr = env_int("D4W_ROW_MAX_RADIX", 25);
@@ -180,8 +182,8 @@ inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, st
             hp.colb_threads = std::min(160, std::max(64, (bmax + 31) / 32 * 32));
             hp.colb_threads = std::min(160, std::max(32, env_int("D4W_COLB_THREADS", hp.colb_threads)));
             {
-                // V chunk = planes * x2 * pairs * 16 B; keep it well inside the 126 MB L2 (D4W_COL_CHUNK_MB = 0: one chunk)
-                const int mb = env_int("D4W_COL_CHUNK_MB", 40);
+                // V chunk = planes * x2 * pairs * 16 B; keep it well inside the H100's 50 MB L2 (D4W_COL_CHUNK_MB = 0: one chunk)
+                const int mb = env_int("D4W_COL_CHUNK_MB", 16);
                 const long long per_pair = (long long)hp.planes * x2 * 16;
                 long long pairs = mb > 0 ? (long long)mb * 1000000 / per_pair / 256 * 256 : (long long)ns / 2;
                 pairs = std::max<long long>(pairs, 256);
@@ -209,8 +211,11 @@ inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, st
             // pipelined single launch: needs the fused level B with (ra, rb) in {(20,20), (16,25)} and 8-pair tiles
             if (env_int("D4W_COL_PIPE", 1) && hp.fused_ra && np == 8 &&
                 ((hp.fused_ra == 20 && hp.fused_rb == 20) || (hp.fused_ra == 16 && hp.fused_rb == 25))) {
-                int cq = env_int("D4W_PIPE_CQ", 80);
-                if (cq < 4 || 160 % cq || (2 * cq) % np) cq = 80;                // strip width in quads; 160 threads = cq x rpc
+                // strip width in quads; 160 threads = cq x rpc.  40 keeps the 4-chunk V ring (13 planes x 400 x 80 pairs x 16 B
+                // = 6.7 MB per chunk, 27 MB in all at 10 000 channels) inside the H100's 50 MB L2; 80 (13.3 MB chunks, a 53 MB
+                // ring) measured 10 % slower
+                int cq = env_int("D4W_PIPE_CQ", 40);
+                if (cq < 4 || 160 % cq || (2 * cq) % np) cq = 40;
                 hp.pipe = 1; hp.pipe_cq = cq; hp.chunk_pairs = 2 * cq;
                 hp.pipe_lag = std::min(256, std::max(1, env_int("D4W_PIPE_LAG", 2)));
                 hp.colb_threads = 160;
@@ -240,7 +245,9 @@ inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, st
     {
         const int nst = hp.rowpl.nstages;
         auto inreg = [](int r) { for (int q : inreg_radices()) if (q == r) return true; return false; };
-        if (!hp.row_dual && env_int("D4W_ROW_FUSED", 1) && nst >= 2 && inreg(hp.rowpl.radix[0]) && inreg(hp.rowpl.radix[nst - 1])) {
+        // f-k filter (default 0): on sm_90 k_row_mid_fused spills at its 128-register cap, and P3 ran 8.6 ms against 2.3 ms
+        // for k_row_mid (H100); the Hilbert plan passes 1, see d4w_row_plan_create
+        if (!hp.row_dual && env_int("D4W_ROW_FUSED", row_fused_default) && nst >= 2 && inreg(hp.rowpl.radix[0]) && inreg(hp.rowpl.radix[nst - 1])) {
             hp.row_fused = 1;
             const int rl = hp.rowpl.radix[nst - 1], G = hp.t2 / rl;
             for (int m = 0; m < rl; ++m)

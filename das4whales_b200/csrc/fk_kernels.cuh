@@ -970,7 +970,7 @@ k_col_inv_dual(ColParams cp, const float2* __restrict__ w, size_t ldw, const int
 
 
 // ================================================================== TMA-fed persistent column kernels
-// Blackwell path for the dominant case (one dual column per tile, ns % 4 == 0): the whole
+// TMA path for the dominant case (one dual column per tile, ns % 4 == 0): the whole
 // [nx x 4 samples] tile moves with 2-D tensor copies (cp.async.bulk.tensor, boxes of 256 rows x 16 B)
 // issued by one thread -- no per-row LSU instruction, completion through an mbarrier (load) or a
 // bulk group (store, fully asynchronous w.r.t. the next tile).  CTAs are persistent (one per SM).

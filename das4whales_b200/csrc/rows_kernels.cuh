@@ -292,8 +292,8 @@ k_xcorr_fused(XcorrParams xp, const float* __restrict__ x, const float2* __restr
 
 // ---- dual-lane variant: FOUR consecutive segments of one channel per CTA as the two f32x2 lanes of the dual engine ---------
 // Element i of the block is the 16-byte cpd {x = (seg_a[i], seg_c[i]), y = (seg_b[i], seg_d[i])}: lane A is the complex
-// signal a + i b, lane B is c + i d, and both lanes run through one instruction stream of packed FFMA2 / FADD2 / FMUL2
-// butterflies (the scalar kernel saturates the FMA pipe at 50 % issue: 3-register FFMA issues every other cycle per SMSP).
+// signal a + i b, lane B is c + i d, and both lanes run through one instruction stream of butterflies whose twiddles are
+// formed once for the two lanes (each lane operation is a scalar FFMA / FADD / FMUL, fft_dual.cuh).
 // The template spectra are lane-independent scalars (dmul_s).  Shared memory: S and B as cpd (16 B x nb each) and the
 // exclusive prefix sums of the mu term as a coarse float4 per 8 samples + an fp16 x 4 remainder per sample (the remainder is
 // a sum of <= 7 normalised samples, |.| <= 7, so its fp16 rounding is <= 4e-3 before the ~1e-6 factor mu / m).

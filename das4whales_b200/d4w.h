@@ -1,4 +1,4 @@
-/* d4w.h -- C ABI of libd4w.so, the B200-native (sm_100a) replacement for the channel-parallel
+/* d4w.h -- C ABI of libd4w.so, the H100-native (sm_90a) replacement for the channel-parallel
  * DSP hot path of DAS4Whales.
  *
  * The reference has no FFI: its boundary is the Python module namespace

@@ -1,6 +1,6 @@
 """das4whales_b200.dsp -- drop-in for the hot-path functions of `das4whales.dsp`
 (/root/reference/src/das4whales/dsp.py), same names / positional order / defaults, running
-on hand-written sm_100a CUDA kernels (libd4w.so) instead of NumPy/SciPy.
+on hand-written sm_90a CUDA kernels (libd4w.so) instead of NumPy/SciPy.
 
 Accepted data: `numpy.ndarray` (any float dtype; the result is a new float64 ndarray, as the
 reference returns) or a CUDA `torch.Tensor` (float32; the result stays on the device).

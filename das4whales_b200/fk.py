@@ -2,7 +2,7 @@
 `FkFilter` object that owns the device buffers.  dsp.fk_filter_design / hybrid_*_filter_design
 return `FkMask`; dsp.fk_filter_filt / fk_filter_sparsefilt run an `FkFilter`.
 
-All arithmetic happens in libd4w.so (hand-written sm_100a CUDA, see csrc/fk_kernels.cuh);
+All arithmetic happens in libd4w.so (hand-written sm_90a CUDA, see csrc/fk_kernels.cuh);
 PyTorch is used for device memory and streams only.
 """
 import threading

@@ -287,9 +287,39 @@ def make_round2():
     return rep
 
 
+def sha256(a):
+    """Digest of a float64 array's C-order bytes: stands in for arrays that are only ever compared for equality."""
+    import hashlib
+    return hashlib.sha256(np.ascontiguousarray(a, dtype="<f8").tobytes()).hexdigest()
+
+
+def make_spot_checks():
+    """tests/golden/spot_checks.npz: the reference's answers on the seeded inputs of the oracle spot checks in
+    tests/test_oracle_golden.py (test_oracle_against_reference, test_round2_oracle_against_reference).  The f-k masks and
+    filter keep the 36 x 200 input of the live-reference checks these replace; the per-row operators (band-pass, correlogram,
+    get_fx) and the image helpers are stored on fewer / shorter rows so that the float64 answers stay a small fixture."""
+    dsp, detect = ref_loader.load()
+    imp = ref_loader.load_improcess()
+    x = np.random.default_rng(5).standard_normal((36, 200))
+    sel = [0, x.shape[0], 1]
+    m = dsp.fk_filter_design(x.shape, sel, DX, FS)
+    tpl = detect.gen_template_fincall(np.arange(x.shape[1]) / FS, FS, 17.8, 28.8, 0.68)
+    sc = dict(fan_mask=m, fan_filt=dsp.fk_filter_filt(x.copy(), m, True),
+              ninf_mask=np.asarray(dsp.hybrid_ninf_filter_design(x.shape, sel, DX, FS)),
+              bp=dsp.bp_filt(x[:8], FS, 14, 30), corr=detect.compute_cross_correlogram(x[:8], tpl))
+    x2 = np.random.default_rng(8).standard_normal((10, 300))
+    img = imp.trace2image(x2)
+    up, down = imp.gabor_filt_design(40.0)
+    sc.update(fx=dsp.get_fx(x2, 256), image=img, binned=imp.binning(img, 0.1, 0.1), gabor_shape=np.array(up.shape),
+              gabor_up_sha256=sha256(up), gabor_down_sha256=sha256(down))
+    np.savez_compressed(os.path.join(OUT, "spot_checks.npz"), **sc)
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "round2":
         for k, v in make_round2().items():
             print(f"{k:24s} oracle-vs-reference rel err {v:.2e}")
+    elif len(sys.argv) > 1 and sys.argv[1] == "spot_checks":
+        make_spot_checks()
     else:
         main()

@@ -35,7 +35,7 @@ def one():
         _lib.lib().d4w_fk_debug_phases(flt.plan.ptr, buf)      # reset
         flt(x, out=y); torch.cuda.synchronize()
         _lib.check(_lib.lib().d4w_fk_debug_phases(flt.plan.ptr, buf), "dbg")
-        nsm = 148
+        nsm = torch.cuda.get_device_properties(x.device).multi_processor_count
         print("phase Mcycles per SM (one apply): fwd load/fft/out =", [round(buf[i] / nsm / 1e6, 3) for i in range(3)],
               " inv drain/fill/fft/store =", [round(buf[i] / nsm / 1e6, 3) for i in range(4, 8)])
     print(json.dumps({"ms": [round(m, 3) for m in ms], "total": round(sum(ms), 3), "err": err,

@@ -1,4 +1,4 @@
-"""CPU: libd4w.so builds for sm_100a, loads, and exports every symbol include/d4w.h declares
+"""CPU: libd4w.so builds for sm_90a, loads, and exports every symbol include/d4w.h declares
 (no compute calls -- there is no GPU here); the product path fails loudly without CUDA."""
 import ctypes
 import os
@@ -42,16 +42,16 @@ def test_no_cpu_fallback():
         dw.detect.compute_cross_correlogram(np.zeros((2, 64)), np.ones(64))
 
 
-def test_sass_is_sm100a(libpath):
-    """The fat binary must contain sm_100a code only (no PTX-JIT or other-arch fallbacks)."""
+def test_sass_is_sm90a(libpath):
+    """The fat binary must contain sm_90a (H100) code only (no PTX-JIT or other-arch fallbacks)."""
     import shutil
     import subprocess
     exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(exe):
         pytest.skip("cuobjdump not available")
     out = subprocess.run([exe, "--list-elf", libpath], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
-    assert all("sm_100a" in line for line in out.splitlines() if "ELF file" in line)
+    assert "sm_90a" in out
+    assert all("sm_90a" in line for line in out.splitlines() if "ELF file" in line)
 
 
 def test_packaged_header_matches_canonical(libpath):

@@ -205,7 +205,8 @@ COLUMN_SCHEMES = [{"D4W_COL_TWO_LEVEL": "0"},                                   
                   {"D4W_COL_PIPE": "0", "D4W_COLB_FUSED": "0"},                 # shared-memory engine level B
                   {"D4W_COLB_RA": "16"},                                        # pipelined, 16 x 25 level B
                   {"D4W_PIPE_CQ": "40", "D4W_PIPE_LAG": "3"},                   # pipelined, narrower chunks / deeper ring
-                  {"D4W_PIPE_HINTS": "0"}]
+                  {"D4W_PIPE_HINTS": "0"},
+                  {"D4W_ROW_FUSED": "1"}]                                       # opt-in fused middle row pass (P3)
 
 
 @pytest.mark.parametrize("env", COLUMN_SCHEMES)

@@ -21,7 +21,7 @@ DX, FS = 2.0419046878814697, 200.0
 
 def _build(name, tmp):
     exe = os.path.join(tmp, name)
-    r = subprocess.run([NVCC, "-std=c++17", "-O2", "--expt-relaxed-constexpr", "-arch=sm_100a",
+    r = subprocess.run([NVCC, "-std=c++17", "-O2", "--expt-relaxed-constexpr", "-arch=sm_90a",
                         "-o", exe, os.path.join(EMUL, name + ".cu")], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr + r.stdout
     return exe
@@ -64,7 +64,8 @@ def _run(exe, tmp, nx, ns, kind, taper, x, kval, fval, c, H=None, dense=None, co
 
 
 CASES = [(40, 240, 1, False, None), (45, 175, 1, True, None), (38, 120, 2, False, None),
-         (100, 1200, 1, True, {"D4W_T1": "12"}), (30, 600, 1, False, {"D4W_T1": "5", "D4W_COL_NC": "1"}),
+         (100, 1200, 1, True, {"D4W_T1": "12"}), (100, 1200, 1, True, {"D4W_T1": "12", "D4W_ROW_FUSED": "1"}),
+         (30, 600, 1, False, {"D4W_T1": "5", "D4W_COL_NC": "1"}),
          (250, 360, 1, False, {"D4W_T1": "6", "D4W_COL_NC": "4"}),
          (10000, 16, 1, False, None),      # the bench column plan (two-level 25 x 400, fused 20 x 20 level B)
          (10000, 10, 1, True, {"D4W_COLB_RA": "16"}), (10000, 8, 1, False, {"D4W_COLB_RA": "25"}),

@@ -77,6 +77,35 @@ def test_snr_golden_and_kat(dw, golden):
         assert rel_err(lin, lref)[0] <= TOL, env
 
 
+HILBERT_ROUTES = [{}, {"D4W_ROW_FUSED": "0"}, {"D4W_HILBERT_PAIR": "0"}, {"D4W_ROW_FUSED": "0", "D4W_HILBERT_PAIR": "0"}]
+
+
+@pytest.mark.parametrize("env", HILBERT_ROUTES)
+def test_envelope_routes_agree(dw, monkeypatch, env):
+    """Every route of the split-row Hilbert transform (two real rows per complex transform or one per row; middle pass
+    k_row_mid_fused, the default here, or k_row_mid) gives the oracle's envelope and SNR, an odd row count included."""
+    from das4whales_b200 import _lib, rows
+    for k, v in env.items():
+        monkeypatch.setenv(k, v)
+    monkeypatch.setattr(rows, "_row_plans", {})                  # plans read the options when they are created
+    nx, ns = 5, 120000
+    x = np.random.default_rng(11).standard_normal((nx, ns)).astype(np.float32)
+    L = _lib.lib()
+    try:
+        env_ = dw.detect.envelope(x)
+        snr = dw.dsp.snr_tr_array(x, env=True)
+        (plan,) = rows._row_plans.values()
+        ws = L.d4w_row_workspace_bytes(plan.ptr, nx)
+    finally:
+        for p in rows._row_plans.values():
+            L.d4w_row_plan_destroy(p.ptr)
+    pair = env.get("D4W_HILBERT_PAIR", "1") != "0"
+    assert ws == ((nx + 1) // 2 if pair else nx) * ns * 8
+    assert rel_err(env_, D.envelope(x.astype(np.float64)))[0] <= 2e-5
+    ref = O.snr_tr_array(x.astype(np.float64), env=True)
+    assert rel_err(10 ** (snr / 10), 10 ** (ref / 10))[0] <= TOL
+
+
 @pytest.mark.parametrize("ns", [600, 12000, 36000, 120000])
 def test_envelope_vs_oracle_lengths(dw, ns):
     rng = np.random.default_rng(ns)
