@@ -219,6 +219,27 @@ def fk_filter_filt(trace, fk_filter_matrix, tapering=False, workers=None):
     return sfft.ifft2(sfft.ifftshift(spec), workers=workers, overwrite_x=True).real
 
 
+def fold_rowmax(mask_shifted):
+    """rowmax[k] = max_f float32(|M_sym[k, f]|) for 0 <= k <= nx/2: the support scan of the opt-in eps pruning."""
+    msym = fold_mask(mask_shifted)
+    return np.abs(msym[: msym.shape[0] // 2 + 1]).astype(np.float32).max(axis=1)
+
+
+def fk_filter_filt_pruned(x, mask_shifted, eps):
+    """The f-k filter with support pruning at threshold eps (FkFilter(mask, eps=eps)): wavenumber row k of the folded
+    mask is kept iff rowmax[k] > float32(eps); otherwise rows k and nx - k of M_sym are zeroed.  Returns
+    (real(ifft2(fft2(x) * M_sym_pruned)), number of kept rows among 0 <= k <= nx/2).  Pruning removes at most eps of
+    every spectral coefficient, so ||y_eps - y||_2 <= eps ||x||_2 (Parseval)."""
+    msym = fold_mask(mask_shifted)
+    nx = msym.shape[0]
+    keep = fold_rowmax(mask_shifted) > np.float32(eps)
+    for k in np.nonzero(~keep)[0]:
+        msym[k] = 0.0
+        msym[(nx - k) % nx] = 0.0
+    y = np.fft.ifft2(np.fft.fft2(np.asarray(x, dtype=np.float64)) * msym).real
+    return y, int(np.count_nonzero(keep))
+
+
 def fk_filter_filt_rows(trace, fk_filter_matrix, rows, cols=None, tapering=False):
     """Same result as fk_filter_filt restricted to output `rows` (all columns) -- used at
     sizes where the full float64 fft2 does not fit in host RAM (SURVEY.md 8d).  Uses the

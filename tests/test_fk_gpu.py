@@ -81,6 +81,46 @@ def test_hybrid_ninf_vs_oracle(dw, nx, ns):
         assert np.max(np.abs(mask.todense() - mref)) <= 1e-12
 
 
+T1_SPLITS = [(24000, 3), (36000, 4), (50000, 5), (60000, 6), (80000, 8), (100000, 10), (120000, 12), (150000, 15),
+             (160000, 16), (200000, 20), (250000, 25)]
+
+
+@pytest.mark.parametrize("ns,t1", T1_SPLITS)
+def test_every_time_split_vs_oracle(dw, ns, t1):
+    """Each length picks its own time split ns = T1 x T2 (T2 <= 10 240), so every k_row_split<T1> instantiation the
+    planner can choose runs on the device (the config-2 length 120 000 is T1 = 12)."""
+    import torch
+    from das4whales_b200 import fk
+    nx = 48
+    assert fk.get_plan(nx, ns, torch.cuda.current_device()).t1 == t1
+    x = np.random.default_rng(ns).standard_normal((nx, ns)).astype(np.float32)
+    sel = [0, nx, 1]
+    y = dw.dsp.fk_filter_filt(x, dw.dsp.fk_filter_design((nx, ns), sel, DX, FS))
+    ref = O.fk_filter_filt(x.astype(np.float64), O.fk_filter_design((nx, ns), sel, DX, FS))
+    e = rel_err(y, ref)
+    assert e[0] <= TOL and e[1] <= TOL, e
+
+
+@pytest.mark.parametrize("nx,scheme", [(48, 0), (200, 2)])
+def test_config2_length_hybrid_tapered_vs_oracle(dw, nx, scheme):
+    """ns = 120 000 (T1 = 12) with the tapered hybrid_ninf mask; at 200 channels the column transform is two-level,
+    25 x 8 with the shared-memory level B."""
+    import torch
+    from das4whales_b200 import fk
+    ns = 120000
+    plan = fk.get_plan(nx, ns, torch.cuda.current_device())
+    assert (plan.t1, plan.col_scheme) == (12, scheme)
+    x = np.random.default_rng(nx).standard_normal((nx, ns)).astype(np.float32)
+    sel, args = [0, nx, 1], (1350., 1450., 3300, 3450, 14., 30.)
+    y = dw.dsp.fk_filter_filt(x.copy(), dw.dsp.hybrid_ninf_filter_design((nx, ns), sel, DX, FS, *args), tapering=True)
+    ref = O.fk_filter_filt(x.astype(np.float64), O.hybrid_ninf_filter_design((nx, ns), sel, DX, FS, *args), tapering=True)
+    e = rel_err(y, ref)
+    assert e[0] <= TOL and e[1] <= TOL, e
+    y = dw.dsp.fk_filter_filt(x, dw.dsp.fk_filter_design((nx, ns), sel, DX, FS))
+    e = rel_err(y, O.fk_filter_filt(x.astype(np.float64), O.fk_filter_design((nx, ns), sel, DX, FS)))
+    assert e[0] <= TOL and e[1] <= TOL, e
+
+
 def test_edge_cases(dw):
     # odd time length breaks the reference's hybrid design the same way (dsp.py:349 broadcast)
     with pytest.raises(ValueError):

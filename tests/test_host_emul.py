@@ -107,6 +107,37 @@ def test_fk_pipeline_emulation(tmpdir_mod):
             assert rel_err(yh, refh)[0] <= 5e-6, (nx, ns, "hybrid_ninf")
 
 
+SUPPORT_CASES = [(40, 240, None), (45, 175, None), (400, 24, None), (320, 12, None),
+                 (10000, 16, None),                                   # two-level 25 x 400, fused 20 x 20 level B
+                 (10000, 8, {"D4W_COLB_FUSED": "0"}), (10000, 8, {"D4W_COL_TWO_LEVEL": "0"}),
+                 (1000, 24, {"D4W_COL_PIPE3": "1", "D4W_PIPE3_CQ": "4", "D4W_PIPE3_THREADS": "32"}),
+                 (6400, 12, {"D4W_COL_X1": "16"}), (8000, 8, {"D4W_COL_X1": "20"})]
+
+
+def test_fk_pipeline_emulation_dense_supports(tmpdir_mod):
+    """Dense masks whose wavenumber support has holes, a single row whose conjugate partner row is empty, or only the
+    DC and Nyquist rows: the kept-row tables of every column scheme (slot positions, two-level plane entries and need
+    tables) against the float64 filter."""
+    exe = _build("fk_pipeline_emul", tmpdir_mod)
+    rng = np.random.default_rng(4)
+    for nx, ns, env in SUPPORT_CASES:
+        x32 = rng.standard_normal((nx, ns)).astype(np.float32)
+        for support in ("scattered", "one_row", "dc_nyquist"):
+            m = rng.standard_normal((nx, ns))                  # signed, not symmetric
+            if support == "scattered":
+                rows = rng.random(nx) < 0.1
+            elif support == "one_row":                         # shifted row nx//2 + 3 is k = 3; row k = -3 stays empty
+                rows = np.arange(nx) == nx // 2 + 3
+            else:                                              # k = 0, and k = -nx/2 (the Nyquist row when nx is even)
+                rows = (np.arange(nx) == nx // 2) | (np.arange(nx) == 0)
+            m[~rows] = 0.0
+            m = m.astype(np.float32).astype(np.float64)
+            ref = O.fk_filter_filt(x32.astype(np.float64), m)
+            y, tail = _run(exe, tmpdir_mod, nx, ns, 2, False, x32, 0.0, 0.0, (0.0,) * 4, dense=m, env=env)
+            assert tail[0] == np.count_nonzero(O.fold_rowmax(m)), (nx, ns, env, support)
+            assert rel_err(y, ref)[0] <= 5e-6, (nx, ns, env, support)
+
+
 def test_peak_picker_emulation(tmpdir_mod):
     """The device peak picker's per-sample body (flat tops, hierarchical prominence walk over 64-sample blocks and
     64-block superblocks) on the host against scipy.signal.find_peaks, index for index, on the same float32 rows."""

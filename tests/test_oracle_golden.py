@@ -190,7 +190,7 @@ def test_round2_gabor_oracle_matches_golden(golden):
 
 
 def test_torch_second_oracle_pinned_to_numpy_oracle():
-    """oracle/torch_oracle.py (the float64 whole-matrix oracle of tests/test_fullsize_gpu.py) == oracle/dsp_oracle.py on the CPU."""
+    """oracle/torch_oracle.py's whole-matrix masks and filter == oracle/dsp_oracle.py on the CPU."""
     import torch
     from oracle import torch_oracle as TO
     rng = np.random.default_rng(3)
@@ -204,6 +204,63 @@ def test_torch_second_oracle_pinned_to_numpy_oracle():
         y = TO.fk_filter_filt(torch.from_numpy(x), torch.from_numpy(mo)).numpy()
         assert rel_err(y, O.fk_filter_filt(x, mo))[0] <= 1e-13
         assert rel_err(O.fk_filter_filt(x, mo, workers=2), O.fk_filter_filt(x, mo))[0] <= 1e-13     # bench's threaded CPU arm
+
+
+@pytest.mark.parametrize("nx,ns", [(36, 200), (37, 201), (40, 150), (33, 242)])
+@pytest.mark.parametrize("tapering", [False, True])
+def test_streaming_torch_oracle_pinned_to_numpy_oracle(nx, ns, tapering):
+    """oracle/torch_oracle.fk_filter_errors (the slab-by-slab float64 oracle of the full-size GPU tests) computes what
+    oracle/dsp_oracle.fk_filter_filt computes, for every mask kind, odd and even shapes, and slabs of a few rows or
+    columns with a ragged last slab; an error planted in y is reported exactly."""
+    import torch
+    from oracle import torch_oracle as TO
+    rng = np.random.default_rng(nx * ns + tapering)
+    sel = [0, nx, 1]
+    x = rng.standard_normal((nx, ns))
+    xt = torch.from_numpy(x.copy())
+    dense = rng.standard_normal((nx, ns)) * (rng.random((nx, 1)) < 0.5)
+    masks = [(O.fk_filter_design((nx, ns), sel, DX, FS), TO.fan_columns((nx, ns), sel, DX, FS)),
+             (dense, TO.dense_columns(torch.from_numpy(dense)))]
+    if ns % 2 == 0:         # the reference's hybrid design needs an even time length (dsp.py:349)
+        args = (1350., 1450., 3300, 3450, 14., 30.)
+        masks.append((O.hybrid_ninf_filter_design((nx, ns), sel, DX, FS, *args),
+                      TO.hybrid_ninf_columns((nx, ns), sel, DX, FS, *args)))
+        j = torch.arange(ns)
+        assert np.max(np.abs(masks[-1][1](j).numpy() - masks[-1][0])) <= 1e-15
+    for m, cols in masks:
+        assert np.max(np.abs(cols(torch.arange(ns)).numpy() - np.asarray(m))) <= 1e-15
+        ref = O.fk_filter_filt(x.copy(), m, tapering=tapering)
+        for rows_per_slab, cols_per_slab in ((5, 7), (nx, ns), (3, 64)):
+            e = TO.fk_filter_errors(xt, torch.from_numpy(ref), cols, tapering=tapering, rows_per_slab=rows_per_slab,
+                                    cols_per_slab=cols_per_slab)
+            assert e.max_norm <= 1e-13 and e.l2 <= 1e-13, e
+            assert abs(e.ref_l2 - np.linalg.norm(ref)) <= 1e-12 * np.linalg.norm(ref)
+            assert abs(e.ref_max - np.max(np.abs(ref))) <= 1e-12 * np.max(np.abs(ref))
+        assert np.array_equal(xt.numpy(), x)
+        bad = ref.copy()
+        bad[nx // 2, ns - 1] += 1e-3 * e.ref_max
+        e = TO.fk_filter_errors(xt, torch.from_numpy(bad), cols, tapering=tapering, rows_per_slab=4, cols_per_slab=50)
+        assert abs(e.max_norm - 1e-3) <= 1e-9 and abs(e.l2 - 1e-3 * e.ref_max / e.ref_l2) <= 1e-9, e
+
+
+def test_pruned_fk_oracle():
+    """oracle/dsp_oracle.fk_filter_filt_pruned: eps = 0 is the exact filter (rows that are zero anyway drop out), the
+    kept-row count follows the row maxima of the folded mask, and the l2 bound ||y_eps - y|| <= eps ||x|| holds."""
+    rng = np.random.default_rng(11)
+    for nx, ns in ((40, 64), (41, 63)):
+        x = rng.standard_normal((nx, ns))
+        m = rng.standard_normal((nx, ns)) * 10.0 ** rng.uniform(-9, 0, (nx, 1))
+        m[rng.random(nx) < 0.3] = 0.0
+        exact = O.fk_filter_filt(x, m)
+        rowmax = O.fold_rowmax(m)
+        y0, kept0 = O.fk_filter_filt_pruned(x, m, 0.0)
+        assert rel_err(y0, exact)[0] <= 1e-13 and kept0 == np.count_nonzero(rowmax > 0)
+        for eps in (1e-7, 1e-4, 1e-2):
+            y, kept = O.fk_filter_filt_pruned(x, m, eps)
+            assert kept == np.count_nonzero(rowmax > np.float32(eps)) and kept < kept0
+            assert np.linalg.norm(y - exact) <= eps * np.linalg.norm(x)
+        k = int(np.argmax(rowmax))
+        assert O.fk_filter_filt_pruned(x, m, float(rowmax[k]))[1] == np.count_nonzero(rowmax > rowmax[k]) < kept0
 
 
 def test_round2_oracle_against_reference(golden):
