@@ -79,7 +79,10 @@ struct d4w_fk_plan {
     size_t colb_smem = 0;
     int colb_threads = 128;
     PipeParams pipe{};                        // pipe.nchunks > 0: single-launch pipelined level A+B
-    FkHostPlan hostplan;                      // kept for mask-time table building
+    int czt = 0;                              // chirp-z column kernels (nx with a prime factor > 61)
+    CztParams cz{};
+    float2 *d_czt_chirp = nullptr, *d_czt_bhat = nullptr;
+    FkHostPlan hostplan;                     // kept for mask-time table building
     std::vector<int> h_k2pos;
     int col_threads = 256, row_threads = 256;
     size_t col_smem = 0, row_smem = 0;
@@ -143,6 +146,10 @@ extern "C" int d4w_fk_plan_create(d4w_fk_plan** out, int nx, int ns, int device)
     if (e == cudaSuccess) e = upload(&pl->d_pos2k_row, p2kr);
     if (e == cudaSuccess) e = upload(&pl->d_taper, tap);
     if (e == cudaSuccess && hp.two_level) e = upload(&pl->d_tw_x2, hp.tw_x2);
+    if (e == cudaSuccess && hp.czt) e = upload(&pl->d_czt_chirp, hp.czt_chirp);
+    if (e == cudaSuccess && hp.czt) e = upload(&pl->d_czt_bhat, hp.czt_bhat);
+    if (e == cudaSuccess && hp.czt) e = cudaFuncSetAttribute(k_col_fwd_czt, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap);
+    if (e == cudaSuccess && hp.czt) e = cudaFuncSetAttribute(k_col_inv_czt, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap);
     if (e == cudaSuccess && env_int("D4W_FK_DEBUG", 0)) { e = cudaMalloc((void**)&pl->d_dbg, 64); if (e == cudaSuccess) e = cudaMemset(pl->d_dbg, 0, 64); }
     // the attribute is per-kernel global state: always raise it to the device maximum, never to a plan's own size
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_col_fwd<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap);
@@ -171,6 +178,14 @@ extern "C" int d4w_fk_plan_create(d4w_fk_plan** out, int nx, int ns, int device)
     }
     pl->col.tw = pl->d_tw_col; pl->col.k2pos = pl->d_k2pos; pl->col.pos2k = pl->d_pos2k;
     pl->row.tw = pl->d_tw_row; pl->row.twT = pl->d_twT;
+    if (hp.czt) {
+        pl->czt = 1;
+        pl->col_threads = 512;
+        CztParams& cz = pl->cz;
+        cz.pl = hp.colpl; cz.tw = pl->d_tw_col; cz.chirp = pl->d_czt_chirp; cz.bhat = pl->d_czt_bhat;
+        cz.nx = nx; cz.ns = ns; cz.m = hp.czt_m;
+        cz.nc = hp.nc; cz.nc_shift = hp.nc_shift; cz.fstride = hp.fstride; cz.aligned = hp.aligned;
+    }
     if (hp.two_level) {
         pl->two_level = 1; pl->colb_smem = hp.colb_smem;
         pl->col2.plb = hp.plb; pl->col2.twb = pl->d_tw_x2; pl->col2.twn = pl->d_tw_col;
@@ -201,6 +216,7 @@ extern "C" int d4w_fk_plan_destroy(d4w_fk_plan* pl) {
     DeviceGuard guard(pl->device);
     cudaFree(pl->d_tw_col); cudaFree(pl->d_tw_row); cudaFree(pl->d_twT);
     cudaFree(pl->d_k2pos); cudaFree(pl->d_pos2k); cudaFree(pl->d_pos2k_row); cudaFree(pl->d_taper); cudaFree(pl->d_dbg); cudaFree(pl->d_tw_x2);
+    cudaFree(pl->d_czt_chirp); cudaFree(pl->d_czt_bhat);
     delete pl;
     return D4W_OK;
 }
@@ -218,7 +234,7 @@ extern "C" int d4w_fk_plan_info(const d4w_fk_plan* pl, int* info) {
     if (!pl || !info) return fail(D4W_ERR_ARG, "d4w_fk_plan_info: null argument");
     info[0] = pl->t1; info[1] = pl->t2; info[2] = 2 * pl->col.nc; info[3] = pl->col.pl.nstages;
     info[4] = pl->row.pl.nstages; info[5] = pl->col_threads; info[6] = pl->row_threads;
-    info[7] = pl->pipe.nchunks ? 3 : pl->two_level ? 2 : pl->col.tma ? 1 : 0;
+    info[7] = pl->czt ? 4 : pl->pipe.nchunks ? 3 : pl->two_level ? 2 : pl->col.tma ? 1 : 0;
     return D4W_OK;
 }
 
@@ -525,6 +541,12 @@ extern "C" int d4w_fk_apply_pass_ex(d4w_fk_plan* pl, d4w_fk_mask* m, const float
         case 1:
             if (!x) return fail(D4W_ERR_ARG, "d4w_fk_apply: null input");
             if (nact == 0) return D4W_OK;
+            if (pl->czt || mp->czt) {
+                if (!(pl->czt && mp->czt)) return fail(D4W_ERR_UNSUPPORTED, "d4w_fk_apply: chirp-z plan mixed with a mixed-radix plan");
+                k_col_fwd_czt<<<ntiles, pl->col_threads, pl->col_smem, stream>>>(pl->cz, x, w, ldw, m->d_slot_pos, nact, tap);
+                D4W_CHECK_LAUNCH("k_col_fwd_czt");
+                return D4W_OK;
+            }
             if (two && ((uintptr_t)x % 16 == 0)) {
                 if (pl->pipe.nchunks && m->d_need) return launch_col2_pipe<false>(pl, m, x, nullptr, v2, w, ldw, tap, stream);
                 for (int tpb = 0; tpb < pl->ns / 2; tpb += pl->col2.vhp) {        // time chunks: V stays in L2 from A to B
@@ -602,6 +624,12 @@ extern "C" int d4w_fk_apply_pass_ex(d4w_fk_plan* pl, d4w_fk_mask* m, const float
             return launch_row_split<true>(pl, w, slot_count, stream);
         case 5:
             if (!y) return fail(D4W_ERR_ARG, "d4w_fk_apply: null output");
+            if (pl->czt || mp->czt) {
+                if (!(pl->czt && mp->czt)) return fail(D4W_ERR_UNSUPPORTED, "d4w_fk_apply: chirp-z plan mixed with a mixed-radix plan");
+                k_col_inv_czt<<<ntiles, pl->col_threads, pl->col_smem, stream>>>(pl->cz, w, ldw, m->d_slot_pos, nact, y);
+                D4W_CHECK_LAUNCH("k_col_inv_czt");
+                return D4W_OK;
+            }
             if (two && ((uintptr_t)y % 16 == 0)) {
                 if (pl->pipe.nchunks && m->d_need) return launch_col2_pipe<true>(pl, m, nullptr, y, v2, w, ldw, nullptr, stream);
                 for (int tpb = 0; tpb < pl->ns / 2; tpb += pl->col2.vhp) {

@@ -109,7 +109,7 @@ inline bool make_plan(int n, int max_radix, FftPlan& pl, std::string& err, int t
     while (t % 3 == 0) t /= 3;
     while (t % 5 == 0) t /= 5;
     if (t != 1) {
-        err = "unsupported FFT length " + std::to_string(n) + ": prime factor > 61 (Bluestein path not built yet)";
+        err = "unsupported FFT length " + std::to_string(n) + ": prime factor > 61";
         return false;
     }
     std::vector<int> smooth;
@@ -158,6 +158,49 @@ inline std::vector<int> make_pos2freq(const FftPlan& pl) {
     std::vector<int> v(pl.n);
     for (int p = 0; p < pl.n; ++p) v[p] = pos_to_freq(pl, p);
     return v;
+}
+
+// true when n has a prime factor above 61, i.e. make_plan cannot build a mixed-radix schedule for it
+inline bool has_prime_factor_above_61(int n) {
+    for (int p = 2; p <= 61 && n > 1; ++p)
+        while (n % p == 0) n /= p;
+    return n > 1;
+}
+
+// smallest 2^a 3^b 5^c >= n
+inline int next_5smooth(int n) {
+    for (int m = std::max(n, 1);; ++m) {
+        int t = m;
+        while (t % 2 == 0) t /= 2;
+        while (t % 3 == 0) t /= 3;
+        while (t % 5 == 0) t /= 5;
+        if (t == 1) return m;
+    }
+}
+
+// forward DFT (exp(-2 pi i jk / n)) in double of a 2^a 3^b 5^c length, recursive decimation in time; host-side
+// table building only (the chirp-z kernel spectrum)
+inline void dft_5smooth_double(std::vector<double>& re, std::vector<double>& im) {
+    const int n = (int)re.size();
+    if (n <= 1) return;
+    const int r = (n % 2 == 0) ? 2 : (n % 3 == 0) ? 3 : 5;
+    const int m = n / r;
+    std::vector<std::vector<double>> sre(r, std::vector<double>(m)), sim(r, std::vector<double>(m));
+    for (int q = 0; q < r; ++q)
+        for (int j = 0; j < m; ++j) { sre[q][j] = re[(size_t)j * r + q]; sim[q][j] = im[(size_t)j * r + q]; }
+    for (int q = 0; q < r; ++q) dft_5smooth_double(sre[q], sim[q]);
+    const double two_pi = 6.283185307179586476925286766559;
+    for (int k = 0; k < n; ++k) {
+        double ar = 0.0, ai = 0.0;
+        for (int q = 0; q < r; ++q) {
+            const long long e = (long long)q * k % n;                 // exact reduction of the twiddle exponent
+            const double a = -two_pi * (double)e / (double)n, c = std::cos(a), s = std::sin(a);
+            const double xr = sre[q][k % m], xi = sim[q][k % m];
+            ar += xr * c - xi * s;
+            ai += xr * s + xi * c;
+        }
+        re[k] = ar; im[k] = ai;
+    }
 }
 
 }  // namespace d4w

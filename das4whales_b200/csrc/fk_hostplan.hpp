@@ -24,6 +24,11 @@ struct FkHostPlan {
     int chunk_pairs = 0;              // sample pairs per level-A/level-B launch pair (V chunk sized to stay in L2)
     int fused_ra = 0, fused_rb = 0;   // level B as a fused two-stage transform (X2 = ra * rb) when both radices are in {16, 20, 25}
     int fused3 = 0, r3[3] = {0, 0, 0};   // X1 = 10 with a three-stage small-radix level B (k_col3_pipe), opt-in: D4W_COL_PIPE3=1
+    // chirp-z column transform (channel counts with a prime factor > 61): colpl is the length-czt_m plan, tw_col its
+    // twiddles, and the single-level kernels' slot positions are natural wavenumbers (pos2k = k2pos = identity)
+    int czt = 0, czt_m = 0;
+    std::vector<float2> czt_chirp;    // c[n] = exp(-i pi (n^2 mod 2 nx) / nx), n < nx
+    std::vector<float2> czt_bhat;     // FFT_M(conj c, wrapped) / M in the M plan's transform order
     FftPlan colpl{}, rowpl{};
     std::vector<float2> tw_col, tw_row, twT;
     std::vector<int> pos2k, k2pos, pos2k_row;
@@ -54,6 +59,54 @@ inline std::vector<float> tukey_window(int m, double alpha) {
     return w;
 }
 
+// Chirp-z (Bluestein) channel transform for an nx with a prime factor > 61:
+//   X[k] = c[k] * sum_n (x[n] c[n]) conj(c[k - n]),   c[n] = exp(-i pi n^2 / nx),
+// the sum being a circular convolution of length M >= 2 nx - 1 (FFT_M -> x B^ -> IFFT_M).  One M-point complex column
+// per time-sample pair must fit the single-level column budget `col_budget` (200 KB on an H100: M <= 25 600, so
+// nx <= 12 800).
+// Largest channel count with a prime factor > 61 whose chirp-z column fits `col_budget` bytes.
+inline int czt_max_channels(size_t col_budget) {
+    int mmax = (int)std::min<size_t>(col_budget / sizeof(float2), 1 << 30);
+    while (mmax > 1 && next_5smooth(mmax) != mmax) --mmax;          // largest 5-smooth M that fits
+    return (mmax + 1) / 2;                                          // every nx with 2 nx - 1 <= M gets an M' <= M
+}
+
+// Fills the column fields of hp for the chirp-z transform; returns 0, or 1 with err set.
+inline int plan_czt_columns(int nx, size_t col_budget, FkHostPlan& hp, std::string& err) {
+    const int m = next_5smooth(2 * nx - 1);
+    if ((size_t)m * sizeof(float2) > col_budget) {
+        err = "channel axis: " + std::to_string(nx) + " channels has a prime factor > 61, and its chirp-z column transform (" +
+              std::to_string(m) + " points) does not fit one SM's column budget: such channel counts are limited to " +
+              std::to_string(czt_max_channels(col_budget)) + "; filter a channel sub-range or decimate the channel axis";
+        return 1;
+    }
+    std::string e2;
+    FftPlan pl;
+    if (!make_plan(m, 25, pl, e2, 256, 16)) { err = "channel axis (chirp-z length " + std::to_string(m) + "): " + e2; return 1; }
+    int nc = 8;                                                      // columns per tile, odd stride between them
+    while (nc > 1 && (size_t)nc * (m | 1) * sizeof(float2) > col_budget) nc >>= 1;
+    hp.czt = 1; hp.czt_m = m; hp.colpl = pl;
+    hp.nc = nc; hp.nc_shift = (nc == 1) ? 0 : (nc == 2) ? 1 : (nc == 4) ? 2 : 3;
+    hp.fstride = nc == 1 ? m : (m | 1); hp.col_smem = (size_t)nc * hp.fstride * sizeof(float2);
+    hp.dual = 0; hp.npair = 0; hp.npair_shift = 0; hp.tma = 0;
+    const double pi = 3.14159265358979323846;
+    const long long two_nx = 2LL * nx;
+    auto phase = [&](long long n) { return pi * (double)((n * n) % two_nx) / (double)nx; };   // exact integer reduction
+    hp.czt_chirp.resize((size_t)nx);
+    for (int n = 0; n < nx; ++n) { const double a = phase(n); hp.czt_chirp[n] = make_float2((float)std::cos(a), (float)(-std::sin(a))); }
+    std::vector<double> re((size_t)m, 0.0), im((size_t)m, 0.0);      // b = conj(c), wrapped: b[j] and b[M - j] = b[-j]
+    for (int j = 0; j < nx; ++j) {
+        const double a = phase(j);
+        re[j] = std::cos(a); im[j] = std::sin(a);
+        if (j > 0) { re[m - j] = re[j]; im[m - j] = im[j]; }
+    }
+    dft_5smooth_double(re, im);
+    const std::vector<int> p2k = make_pos2freq(pl);
+    hp.czt_bhat.resize((size_t)m);
+    for (int p = 0; p < m; ++p) hp.czt_bhat[p] = make_float2((float)(re[p2k[p]] / m), (float)(im[p2k[p]] / m));
+    return 0;
+}
+
 inline const std::vector<int>& split_radices() {
     static const std::vector<int> r = {1, 2, 3, 4, 5, 6, 8, 10, 12, 15, 16, 20, 25};
     return r;
@@ -72,7 +125,8 @@ inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, st
     while (nc > 1 && (size_t)nc * (nx + 1) * sizeof(float2) > col_budget) nc >>= 1;
     if ((size_t)nc * (nx + 1) * sizeof(float2) > smem_cap) {
         err = "channel axis too long (" + std::to_string(nx) + " channels): one column of the wavenumber transform must fit one SM's "
-              "shared memory (about 28 000 channels); filter a channel sub-range or decimate the channel axis";
+              "shared memory (about 28 000 channels, " + std::to_string(czt_max_channels(col_budget)) +
+              " when the count has a prime factor > 61); filter a channel sub-range or decimate the channel axis";
         return 1;
     }
     const int forced_nc = env_int("D4W_COL_NC", 0);
@@ -94,7 +148,10 @@ inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, st
     if (hp.tma) { hp.fstride = (nx + 255) / 256 * 256; hp.col_smem = (size_t)hp.fstride * 16; }
     const char* col_spec = std::getenv("D4W_COL_PLAN");
     if (!(col_spec && *col_spec && make_plan_from_string(nx, col_spec, hp.colpl)) &&
-        !make_plan(nx, hp.dual ? std::min(col_maxr, env_int("D4W_DUAL_MAX_RADIX", 25)) : col_maxr, hp.colpl, e2, 256, hp.dual ? 8 : 16)) { err = "channel axis: " + e2; return 1; }
+        !make_plan(nx, hp.dual ? std::min(col_maxr, env_int("D4W_DUAL_MAX_RADIX", 25)) : col_maxr, hp.colpl, e2, 256, hp.dual ? 8 : 16)) {
+        if (!has_prime_factor_above_61(nx)) { err = "channel axis: " + e2; return 1; }
+        if (plan_czt_columns(nx, col_budget, hp, err)) return 1;       // single-level chirp-z column kernels only
+    }
 
     // time axis = T1 (registers) x T2 (shared memory).  Dual-lane row kernel (default): T2 <= 6144 keeps the
     // 16-byte-element tile under 96 KB -> two CTAs per SM; scalar kernel: T2 <= 10240 (16384 when T1 == 1).
@@ -135,7 +192,7 @@ inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, st
         return 1;
     }
     // ---- small-radix variant: X1 = 10 in registers, X2 = R0*R1*R2 with radices <= 10 (three-stage level B), single pipelined launch
-    if (env_int("D4W_COL_TWO_LEVEL", 1) && env_int("D4W_COL_PIPE3", 0) && ns % 4 == 0 && nx % 10 == 0) {
+    if (!hp.czt && env_int("D4W_COL_TWO_LEVEL", 1) && env_int("D4W_COL_PIPE3", 0) && ns % 4 == 0 && nx % 10 == 0) {
         const int x2 = nx / 10;
         static const int cand[][3] = {{10, 10, 10}, {5, 5, 4}};
         for (auto& c : cand) {
@@ -162,7 +219,7 @@ inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, st
         }
     }
     // ---- two-level column split: X1 in registers (largest of 25, 20, 16), X2-point smem FFT
-    if (!hp.fused3 && env_int("D4W_COL_TWO_LEVEL", 1) && ns % 4 == 0) {
+    if (!hp.czt && !hp.fused3 && env_int("D4W_COL_TWO_LEVEL", 1) && ns % 4 == 0) {
         const int forced_x1 = env_int("D4W_COL_X1", 0);
         for (int cand : {25, 20, 16}) {
             if (forced_x1 && cand != forced_x1) continue;
@@ -230,14 +287,19 @@ inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, st
     for (int st = 0; st < hp.colpl.nstages; ++st) hp.col_max_radix = std::max(hp.col_max_radix, hp.colpl.radix[st]);
     hp.t1 = t1; hp.t2 = ns / t1;
     hp.row_smem = (size_t)hp.t2 * (hp.row_dual ? 16 : sizeof(float2));
-    hp.tw_col = make_twiddles(nx);
+    hp.tw_col = make_twiddles(hp.czt ? hp.czt_m : nx);
     hp.tw_row = make_twiddles(hp.t2);
     hp.twT.resize((size_t)hp.t2);
     for (int j = 0; j < hp.t2; ++j) {
         const double a = 6.283185307179586476925286766559 * (double)j / (double)ns;
         hp.twT[j] = make_float2((float)std::cos(a), (float)(-std::sin(a)));
     }
-    hp.pos2k = make_pos2freq(hp.colpl);
+    if (hp.czt) {                     // the chirp-z column leaves wavenumbers in natural order
+        hp.pos2k.resize((size_t)nx);
+        for (int p = 0; p < nx; ++p) hp.pos2k[p] = p;
+    } else {
+        hp.pos2k = make_pos2freq(hp.colpl);
+    }
     hp.k2pos.assign((size_t)nx, 0);
     for (int p = 0; p < nx; ++p) hp.k2pos[hp.pos2k[p]] = p;
     hp.pos2k_row = make_pos2freq(hp.rowpl);

@@ -381,6 +381,123 @@ __host__ __device__ inline void body_col_inv_dual(const ColParams& cp, const flo
     }
 }
 
+// ================================================================== chirp-z column passes (nx with a prime factor > 61)
+// X[k] = c[k] * sum_n (x[n] c[n]) b[k - n] with c[n] = exp(-i pi n^2 / nx) and b = conj(c): the sum is a circular
+// convolution of length M >= 2 nx - 1, done as FFT_M -> x bhat -> IFFT_M with the shared-memory engine (bhat = FFT_M(b) / M
+// in transform order, so no reordering).  The inverse DFT is the same with every chirp conjugated (bhat -> conj bhat, as
+// b is even).  Same tile (2*nc time samples, nc complex columns) and kept-row slot layout as body_col_fwd / body_col_inv;
+// slot_pos holds natural wavenumbers (k, nx - k).
+struct CztParams {
+    FftPlan pl;            // length M
+    const float2* tw;      // W_M^j
+    const float2* chirp;   // c[n], n < nx
+    const float2* bhat;    // FFT_M(b) / M, transform order
+    int nx, ns, m;
+    int nc, nc_shift, fstride, aligned;
+};
+
+__host__ __device__ inline void czt_convolve(const CztParams& cp, float2* smem, bool conj_kernel, int tid, int nthr) {
+    const int nc = cp.nc, sh = cp.nc_shift;
+    fft_forward_stages(smem, cp.pl, cp.tw, nc, cp.fstride, tid, nthr, 0, cp.pl.nstages);
+    for (int i = tid; i < (cp.m << sh); i += nthr) {
+        const int p = i >> sh, col = i & (nc - 1);
+        float2& v = smem[col * cp.fstride + p];
+        v = conj_kernel ? cmulc(v, cp.bhat[p]) : cmul(v, cp.bhat[p]);
+    }
+    D4W_SYNC();
+    fft_inverse_stages(smem, cp.pl, cp.tw, nc, cp.fstride, tid, nthr, 0, cp.pl.nstages);
+}
+
+__host__ __device__ inline void body_col_fwd_czt(const CztParams& cp, const float* __restrict__ x, float2* __restrict__ w,
+                                                 size_t ldw, const int2* __restrict__ slot_pos, int nact,
+                                                 const float* __restrict__ taper, int bx, int tid, int nthr, float2* smem) {
+    const int nc = cp.nc, sh = cp.nc_shift, ns = cp.ns, nx = cp.nx;
+    const int t0 = bx * 2 * nc;
+    // two real time columns as one complex column z = x_t + i x_{t+1}, tapered, times c[n], zero-padded to M
+    for (int i = tid; i < (cp.m << sh); i += nthr) {
+        const int c = i >> sh, col = i & (nc - 1);
+        const int t = t0 + 2 * col;
+        float a = 0.f, b = 0.f;
+        if (c < nx) {
+            const float* row = x + (size_t)c * ns;
+            if (t + 1 < ns) {
+                if (cp.aligned) { const float2 v = *reinterpret_cast<const float2*>(row + t); a = v.x; b = v.y; }
+                else { a = row[t]; b = row[t + 1]; }
+                if (taper) { a *= taper[t]; b *= taper[t + 1]; }
+            } else if (t < ns) {
+                a = row[t];
+                if (taper) a *= taper[t];
+            }
+        }
+        smem[col * cp.fstride + c] = c < nx ? cmul(make_float2(a, b), cp.chirp[c]) : make_float2(0.f, 0.f);
+    }
+    D4W_SYNC();
+    czt_convolve(cp, smem, false, tid, nthr);
+    // Z[k] = c[k] * conv[k]; two-for-one untangle as in body_col_fwd
+    for (int i = tid; i < (nact << sh); i += nthr) {
+        const int slot = i >> sh, col = i & (nc - 1);
+        const int2 pp = slot_pos[slot];
+        const float2 z = cmul(smem[col * cp.fstride + pp.x], cp.chirp[pp.x]);
+        const float2 z2 = cmul(smem[col * cp.fstride + pp.y], cp.chirp[pp.y]);
+        const float2 xa = make_float2(0.5f * (z.x + z2.x), 0.5f * (z.y - z2.y));   // (z + conj z2)/2
+        const float2 xb = make_float2(0.5f * (z.y + z2.y), 0.5f * (z2.x - z.x));   // (z - conj z2)/(2i)
+        const int t = t0 + 2 * col;
+        float2* o = w + (size_t)slot * ldw + t;
+        if (cp.aligned && t + 1 < ns) {
+            *reinterpret_cast<float4*>(o) = make_float4(xa.x, xa.y, xb.x, xb.y);
+        } else {
+            if (t < ns) o[0] = xa;
+            if (t + 1 < ns) o[1] = xb;
+        }
+    }
+}
+
+__host__ __device__ inline void body_col_inv_czt(const CztParams& cp, const float2* __restrict__ w, size_t ldw,
+                                                 const int2* __restrict__ slot_pos, int nact, float* __restrict__ y, int bx,
+                                                 int tid, int nthr, float2* smem) {
+    const int nc = cp.nc, sh = cp.nc_shift, ns = cp.ns, nx = cp.nx;
+    const int t0 = bx * 2 * nc;
+    // pruned rows (and the padding up to M) are zero
+    for (int i = tid; i < nc * cp.fstride; i += nthr) smem[i] = make_float2(0.f, 0.f);
+    D4W_SYNC();
+    // Z[k] = Y_t[k] + i Y_{t+1}[k] over the full k range (Hermitian partners k -> nx - k), times conj(c[k])
+    for (int i = tid; i < (nact << sh); i += nthr) {
+        const int slot = i >> sh, col = i & (nc - 1);
+        const int2 pp = slot_pos[slot];
+        const int t = t0 + 2 * col;
+        const float2* src = w + (size_t)slot * ldw + t;
+        float2 y0 = make_float2(0.f, 0.f), y1 = make_float2(0.f, 0.f);
+        if (cp.aligned && t + 1 < ns) {
+            const float4 v = *reinterpret_cast<const float4*>(src);
+            y0 = make_float2(v.x, v.y); y1 = make_float2(v.z, v.w);
+        } else {
+            if (t < ns) y0 = src[0];
+            if (t + 1 < ns) y1 = src[1];
+        }
+        if (pp.x == pp.y) {                                   // self-conjugate rows (k = 0, nx/2) are real
+            smem[col * cp.fstride + pp.x] = cmulc(make_float2(y0.x, y1.x), cp.chirp[pp.x]);
+        } else {
+            smem[col * cp.fstride + pp.x] = cmulc(make_float2(y0.x - y1.y, y0.y + y1.x), cp.chirp[pp.x]);
+            smem[col * cp.fstride + pp.y] = cmulc(make_float2(y0.x + y1.y, y1.x - y0.y), cp.chirp[pp.y]);
+        }
+    }
+    D4W_SYNC();
+    czt_convolve(cp, smem, true, tid, nthr);
+    // z[n] = conj(c[n]) * conv[n]: real part -> sample t, imaginary part -> t + 1
+    for (int i = tid; i < (nx << sh); i += nthr) {
+        const int c = i >> sh, col = i & (nc - 1);
+        const float2 z = cmulc(smem[col * cp.fstride + c], cp.chirp[c]);
+        const int t = t0 + 2 * col;
+        float* row = y + (size_t)c * ns;
+        if (t + 1 < ns) {
+            if (cp.aligned) *reinterpret_cast<float2*>(row + t) = z;
+            else { row[t] = z.x; row[t + 1] = z.y; }
+        } else if (t < ns) {
+            row[t] = z.x;
+        }
+    }
+}
+
 // ------------------------------------------------------------------ P2 / P4: radix-T1 time split (registers only)
 template <int T1, bool INV>
 __host__ __device__ inline void body_row_split(float2* __restrict__ w, size_t ldw, int t2len, const float2* __restrict__ twT,
@@ -952,6 +1069,18 @@ static __global__ void __launch_bounds__(MAXT, 1)
 k_col_inv(ColParams cp, const float2* __restrict__ w, size_t ldw, const int2* __restrict__ slot_pos, int nact,
           float* __restrict__ y) {
     body_col_inv(cp, w, ldw, slot_pos, nact, y, blockIdx.x, threadIdx.x, blockDim.x, d4w_dyn_smem);
+}
+
+static __global__ void __launch_bounds__(512, 1)
+k_col_fwd_czt(CztParams cp, const float* __restrict__ x, float2* __restrict__ w, size_t ldw, const int2* __restrict__ slot_pos,
+              int nact, const float* __restrict__ taper) {
+    body_col_fwd_czt(cp, x, w, ldw, slot_pos, nact, taper, blockIdx.x, threadIdx.x, blockDim.x, d4w_dyn_smem);
+}
+
+static __global__ void __launch_bounds__(512, 1)
+k_col_inv_czt(CztParams cp, const float2* __restrict__ w, size_t ldw, const int2* __restrict__ slot_pos, int nact,
+              float* __restrict__ y) {
+    body_col_inv_czt(cp, w, ldw, slot_pos, nact, y, blockIdx.x, threadIdx.x, blockDim.x, d4w_dyn_smem);
 }
 
 template <int MAXT>

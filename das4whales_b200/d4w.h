@@ -47,7 +47,8 @@ int d4w_fk_plan_destroy(d4w_fk_plan* plan);
 /* describe the plan: info[0]=T1 (row split), [1]=T2, [2]=column tile width in samples,
  * [3]=column stages, [4]=row stages, [5]=column threads, [6]=row threads,
  * [7]=column scheme: 0 single-level cp.async, 1 single-level TMA, 2 two-level (X1 in registers, X2 fused two-stage),
- *      3 two-level as one pipelined launch per direction (intermediate kept in L2) */
+ *      3 two-level as one pipelined launch per direction (intermediate kept in L2),
+ *      4 chirp-z single-level (nx with a prime factor > 61, nx <= 12 800; [3] counts the stages of the M-point transform) */
 int d4w_fk_plan_info(const d4w_fk_plan* plan, int* info8);
 /* profiling aid (plan created with env D4W_FK_DEBUG=1): summed SM cycles per phase of the TMA column
  * kernels since the last call -- [0..2] forward: load wait, FFT, untangle+store; [4..7] inverse: store

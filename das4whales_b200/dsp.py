@@ -326,10 +326,17 @@ def snr_tr_array(trace, env=False):
     return y if _is_tensor(trace) else _to_host64(y)
 
 
+# Channel counts with a prime factor > 61 go through the chirp-z column transform of length M = the smallest 2^a 3^b 5^c
+# >= 2 nx - 1, and one M-point complex column must fit the 200 KB column budget: M <= 25 600, so nx <= 12 800
+# (csrc/fk_hostplan.hpp, czt_max_channels).
+CZT_MAX_CHANNELS = 12800
+
+
 def supported_shape(nx, ns):
-    """Largest (nx', ns') <= (nx, ns) the f-k / row FFT planner accepts.  The GPU transforms are mixed-radix: every prime factor
-    must be <= 61, the time axis must split as ns = T1 * T2 with T1 <= 25 and T2 <= 10 240, and one channel column must fit an
-    SM's shared memory (about 28 000 channels).  numpy.fft takes any length; crop (or pad the record before loading) to the
+    """Largest (nx', ns') <= (nx, ns) the f-k / row FFT planner accepts.  The f-k filter takes any channel count up to
+    12 800; above that the channel count must have no prime factor > 61 and one channel column must fit an SM's shared
+    memory (about 28 000 channels).  The time axis is mixed-radix: every prime factor must be <= 61 and it must split as
+    ns = T1 * T2 with T1 <= 25 and T2 <= 10 240.  numpy.fft takes any length; crop (or pad the record before loading) to the
     suggested shape when `fk_filter_filt` / `envelope` raise ValueError for an unsupported length."""
     def smooth(n):
         for p in (2, 3, 5, 7, 11, 13, 17, 19, 23, 29, 31, 37, 41, 43, 47, 53, 59, 61):
@@ -342,7 +349,7 @@ def supported_shape(nx, ns):
             return False
         return any(n % t1 == 0 and n // t1 <= (16384 if t1 == 1 else 10240) for t1 in (1, 2, 3, 4, 5, 6, 8, 10, 12, 15, 16, 20, 25))
     nx2 = min(int(nx), 28000)
-    while nx2 > 1 and not smooth(nx2):
+    while nx2 > CZT_MAX_CHANNELS and not smooth(nx2):
         nx2 -= 1
     ns2 = int(ns)
     while ns2 > 1 and not time_ok(ns2):

@@ -42,6 +42,7 @@ class _Plan:
         info = _lib.ffi.new("int[8]")
         _lib.check(L.d4w_fk_plan_info(self.ptr, info), "fk plan info")
         self.t1, self.t2, self.tile, self.col_stages, self.row_stages = info[0], info[1], info[2], info[3], info[4]
+        # column transform: 0 single-level, 1 single-level TMA, 2 two-level, 3 pipelined two-level, 4 chirp-z single-level
         self.col_scheme = int(info[7])
         self.workspace = None
 
