@@ -182,7 +182,37 @@ struct d4w_row_plan {
     float* d_sgn = nullptr;      // sgn(f)/ns in k_row_mid_fused's table order (two-rows-per-transform route)
     size_t row_smem = 0;
     int fused = 0;               // split rows: middle pass by k_row_mid_fused (weights stored in its table order)
+    // chirp-z rows (no mixed-radix split of ns): t1 x t2 = czt_m is the convolution length, hilbert_czt.cuh
+    int czt_m = 0, pair = 0;
+    float2 *d_chirp = nullptr, *d_bhat = nullptr, *d_bhatc = nullptr;
 };
+
+// plan for a row length the time-axis planner rejects: chirp-z transform over an m-point convolution
+static int row_plan_create_czt(d4w_row_plan** out, int ns, int device, const cudaDeviceProp& prop) {
+    RowCztPlan cz; std::string err;
+    if (plan_czt_rows(ns, prop.sharedMemPerBlockOptin, cz, err)) return fail(D4W_ERR_UNSUPPORTED, err);
+    const FkHostPlan& hp = cz.hp;
+    auto p = new d4w_row_plan();
+    p->ns = ns; p->device = device; p->t1 = hp.t1; p->t2 = hp.t2; p->row_smem = hp.row_smem;
+    p->row.pl = hp.rowpl; p->row.t1 = hp.t1; p->row.t2 = hp.t2;
+    p->fused = cz.fused; p->czt_m = cz.m;
+    p->pair = (hp.t1 > 1 && env_int("D4W_HILBERT_PAIR", 1)) ? 1 : 0;
+    std::vector<float2> bc(cz.bhat.size());
+    for (size_t i = 0; i < bc.size(); ++i) bc[i] = make_float2(cz.bhat[i].x, -cz.bhat[i].y);
+    cudaError_t e = upload(&p->d_tw, hp.tw_row);
+    if (e == cudaSuccess) e = upload(&p->d_twT, hp.twT);
+    if (e == cudaSuccess) e = upload(&p->d_chirp, cz.chirp);
+    if (e == cudaSuccess) e = upload(&p->d_bhat, cz.bhat);
+    if (e == cudaSuccess) e = upload(&p->d_bhatc, bc);
+    const int smax = (int)prop.sharedMemPerBlockOptin;
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_row_mid_c, cudaFuncAttributeMaxDynamicSharedMemorySize, smax);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_row_mid_fused_c, cudaFuncAttributeMaxDynamicSharedMemorySize, smax);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_hczt_row, cudaFuncAttributeMaxDynamicSharedMemorySize, smax);
+    if (e != cudaSuccess) { d4w_row_plan_destroy(p); return fail(D4W_ERR_CUDA, std::string("row plan: ") + cudaGetErrorString(e)); }
+    p->row.tw = p->d_tw; p->row.twT = p->d_twT;
+    *out = p;
+    return D4W_OK;
+}
 
 extern "C" int d4w_row_plan_create(d4w_row_plan** out, int ns, int device) {
     if (!out) return fail(D4W_ERR_ARG, "d4w_row_plan_create: null output");
@@ -194,8 +224,9 @@ extern "C" int d4w_row_plan_create(d4w_row_plan** out, int ns, int device) {
     FkHostPlan hp; std::string err;
     // the envelope keeps k_row_mid_fused: 10 000 x 120 000 on an H100 took 15.5 ms with it and 16.9 ms with k_row_mid
     // (two rows per transform both ways; one row per transform: 25.1 ms)
+    // a length with no T1 x T2 split (a prime factor > 61, or T2 too long) goes through the chirp-z rows
     if (build_fk_hostplan(1, ns, prop.sharedMemPerBlockOptin, hp, err, /*allow_row_dual=*/false, /*row_fused_default=*/1))
-        return fail(D4W_ERR_UNSUPPORTED, err);
+        return row_plan_create_czt(out, ns, device, prop);
     auto p = new d4w_row_plan();
     p->ns = ns; p->device = device; p->t1 = hp.t1; p->t2 = hp.t2; p->row_smem = hp.row_smem;
     p->row.pl = hp.rowpl; p->row.t1 = hp.t1; p->row.t2 = hp.t2;
@@ -234,14 +265,71 @@ extern "C" int d4w_row_plan_destroy(d4w_row_plan* p) {
     if (!p) return D4W_OK;
     DeviceGuard guard(p->device);
     cudaFree(p->d_tw); cudaFree(p->d_twT); cudaFree(p->d_hilbert); cudaFree(p->d_sgn);
+    cudaFree(p->d_chirp); cudaFree(p->d_bhat); cudaFree(p->d_bhatc);
     delete p;
     return D4W_OK;
 }
 
 extern "C" size_t d4w_row_workspace_bytes(const d4w_row_plan* p, int nx) {
     if (!p || p->t1 == 1) return 16;
-    const size_t rows = p->d_sgn ? (size_t)(nx + 1) / 2 : (size_t)nx;      // two real rows share one complex workspace row
-    return rows * p->ns * sizeof(float2);
+    const bool pair = p->czt_m ? p->pair != 0 : p->d_sgn != nullptr;
+    const size_t rows = pair ? (size_t)(nx + 1) / 2 : (size_t)nx;      // two real rows share one complex workspace row
+    return rows * (size_t)(p->czt_m ? p->czt_m : p->ns) * sizeof(float2);
+}
+
+extern "C" int d4w_row_plan_info(const d4w_row_plan* p, int* t1, int* t2, int* czt_m) {
+    if (!p) return fail(D4W_ERR_ARG, "d4w_row_plan_info: null plan");
+    if (t1) *t1 = p->t1;
+    if (t2) *t2 = p->t2;
+    if (czt_m) *czt_m = p->czt_m;
+    return D4W_OK;
+}
+
+// chirp-z rows: one CTA per row (t1 == 1), or the five split launches of hilbert_czt.cuh
+static int hilbert_czt(d4w_row_plan* p, const float* x, float* out, int nx, void* workspace, int mode, const double* dev_stats,
+                       cudaStream_t stream) {
+    HcztParams hz{};
+    hz.n = p->ns; hz.m = p->czt_m; hz.t2 = p->t2; hz.nx = nx; hz.pair = p->pair; hz.invn = (float)(1.0 / p->ns);
+    hz.chirp = p->d_chirp; hz.twT = p->d_twT;
+    if (p->t1 == 1) {
+        k_hczt_row<<<nx, 256, p->row_smem, stream>>>(p->row, hz, p->d_bhat, p->d_bhatc, x, out, mode, dev_stats);
+        D4W_CHECK_LAUNCH("k_hczt_row");
+        return D4W_OK;
+    }
+    if (!workspace) return fail(D4W_ERR_ARG, "d4w_hilbert: workspace required for split rows");
+    float2* w = (float2*)workspace;
+    const int nrow = p->pair ? (nx + 1) / 2 : nx, thr = 128;
+    const dim3 g((p->t2 + thr - 1) / thr, nrow), gm(p->t1, nrow);
+    auto mid = [&](const float2* tab) {
+        if (p->fused) k_row_mid_fused_c<<<gm, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->czt_m, tab, (size_t)0);
+        else k_row_mid_c<<<gm, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->czt_m, tab, (size_t)0);
+    };
+    switch (p->t1) {
+#define D4W_HC(T) case T: k_hczt_fwd<T><<<g, thr, 0, stream>>>(hz, x, w); break;
+        D4W_HC(2) D4W_HC(3) D4W_HC(4) D4W_HC(5) D4W_HC(6) D4W_HC(8) D4W_HC(10) D4W_HC(12) D4W_HC(15) D4W_HC(16) D4W_HC(20) D4W_HC(25)
+#undef D4W_HC
+        default: return fail(D4W_ERR_UNSUPPORTED, "row split radix not built");
+    }
+    D4W_CHECK_LAUNCH("k_hczt_fwd");
+    mid(p->d_bhat);
+    D4W_CHECK_LAUNCH("k_row_mid_c");
+    switch (p->t1) {
+#define D4W_HC(T) case T: k_hczt_turn<T><<<g, thr, 0, stream>>>(hz, w); break;
+        D4W_HC(2) D4W_HC(3) D4W_HC(4) D4W_HC(5) D4W_HC(6) D4W_HC(8) D4W_HC(10) D4W_HC(12) D4W_HC(15) D4W_HC(16) D4W_HC(20) D4W_HC(25)
+#undef D4W_HC
+        default: return fail(D4W_ERR_UNSUPPORTED, "row split radix not built");
+    }
+    D4W_CHECK_LAUNCH("k_hczt_turn");
+    mid(p->d_bhatc);
+    D4W_CHECK_LAUNCH("k_row_mid_c");
+    switch (p->t1) {
+#define D4W_HC(T) case T: k_hczt_inv<T><<<g, thr, 0, stream>>>(hz, w, x, out, mode, dev_stats); break;
+        D4W_HC(2) D4W_HC(3) D4W_HC(4) D4W_HC(5) D4W_HC(6) D4W_HC(8) D4W_HC(10) D4W_HC(12) D4W_HC(15) D4W_HC(16) D4W_HC(20) D4W_HC(25)
+#undef D4W_HC
+        default: return fail(D4W_ERR_UNSUPPORTED, "row split radix not built");
+    }
+    D4W_CHECK_LAUNCH("k_hczt_inv");
+    return D4W_OK;
 }
 
 extern "C" int d4w_hilbert(d4w_row_plan* p, const float* x, float* out, int nx, void* workspace, int mode,
@@ -252,6 +340,7 @@ extern "C" int d4w_hilbert(d4w_row_plan* p, const float* x, float* out, int nx, 
     if (nx > 65535 && p->t1 > 1) return fail(D4W_ERR_UNSUPPORTED, "d4w_hilbert: more than 65535 rows per call");
     DeviceGuard guard(p->device);
     cudaStream_t stream = (cudaStream_t)stream_v;
+    if (p->czt_m) return hilbert_czt(p, x, out, nx, workspace, mode, dev_stats, stream);
     if (p->t1 == 1) {
         k_hilbert_row<<<nx, 256, p->row_smem, stream>>>(p->row, x, out, p->d_hilbert, mode, dev_stats);
         D4W_CHECK_LAUNCH("k_hilbert_row");

@@ -71,6 +71,27 @@ inline int czt_max_channels(size_t col_budget) {
     return (mmax + 1) / 2;                                          // every nx with 2 nx - 1 <= M gets an M' <= M
 }
 
+// Chirp and kernel-spectrum tables of a length-n chirp-z transform over an m-point convolution (m >= 2 n - 1):
+// chirp[j] = c[j] = exp(-i pi (j^2 mod 2n) / n) for j < n (exact 64-bit reduction of the phase), and
+// bhat[p] = FFT_m(conj c, wrapped)[tab2freq[p]] / m, computed in double and rounded to fp32 once.  tab2freq maps each
+// table entry to its frequency, i.e. the order in which the consuming kernel reads the spectrum.
+inline void czt_tables(int n, int m, const std::vector<int>& tab2freq, std::vector<float2>& chirp, std::vector<float2>& bhat) {
+    const double pi = 3.14159265358979323846;
+    const long long two_n = 2LL * n;
+    auto phase = [&](long long j) { return pi * (double)((j * j) % two_n) / (double)n; };   // exact integer reduction
+    chirp.resize((size_t)n);
+    for (int j = 0; j < n; ++j) { const double a = phase(j); chirp[j] = make_float2((float)std::cos(a), (float)(-std::sin(a))); }
+    std::vector<double> re((size_t)m, 0.0), im((size_t)m, 0.0);      // b = conj(c), wrapped: b[j] and b[M - j] = b[-j]
+    for (int j = 0; j < n; ++j) {
+        const double a = phase(j);
+        re[j] = std::cos(a); im[j] = std::sin(a);
+        if (j > 0) { re[m - j] = re[j]; im[m - j] = im[j]; }
+    }
+    dft_5smooth_double(re, im);
+    bhat.resize((size_t)m);
+    for (int p = 0; p < m; ++p) bhat[p] = make_float2((float)(re[tab2freq[p]] / m), (float)(im[tab2freq[p]] / m));
+}
+
 // Fills the column fields of hp for the chirp-z transform; returns 0, or 1 with err set.
 inline int plan_czt_columns(int nx, size_t col_budget, FkHostPlan& hp, std::string& err) {
     const int m = next_5smooth(2 * nx - 1);
@@ -89,21 +110,7 @@ inline int plan_czt_columns(int nx, size_t col_budget, FkHostPlan& hp, std::stri
     hp.nc = nc; hp.nc_shift = (nc == 1) ? 0 : (nc == 2) ? 1 : (nc == 4) ? 2 : 3;
     hp.fstride = nc == 1 ? m : (m | 1); hp.col_smem = (size_t)nc * hp.fstride * sizeof(float2);
     hp.dual = 0; hp.npair = 0; hp.npair_shift = 0; hp.tma = 0;
-    const double pi = 3.14159265358979323846;
-    const long long two_nx = 2LL * nx;
-    auto phase = [&](long long n) { return pi * (double)((n * n) % two_nx) / (double)nx; };   // exact integer reduction
-    hp.czt_chirp.resize((size_t)nx);
-    for (int n = 0; n < nx; ++n) { const double a = phase(n); hp.czt_chirp[n] = make_float2((float)std::cos(a), (float)(-std::sin(a))); }
-    std::vector<double> re((size_t)m, 0.0), im((size_t)m, 0.0);      // b = conj(c), wrapped: b[j] and b[M - j] = b[-j]
-    for (int j = 0; j < nx; ++j) {
-        const double a = phase(j);
-        re[j] = std::cos(a); im[j] = std::sin(a);
-        if (j > 0) { re[m - j] = re[j]; im[m - j] = im[j]; }
-    }
-    dft_5smooth_double(re, im);
-    const std::vector<int> p2k = make_pos2freq(pl);
-    hp.czt_bhat.resize((size_t)m);
-    for (int p = 0; p < m; ++p) hp.czt_bhat[p] = make_float2((float)(re[p2k[p]] / m), (float)(im[p2k[p]] / m));
+    czt_tables(nx, m, make_pos2freq(pl), hp.czt_chirp, hp.czt_bhat);
     return 0;
 }
 
@@ -317,6 +324,44 @@ inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, st
         }
     }
     hp.taper = tukey_window(ns, 0.03);
+    return 0;
+}
+
+// ---- Hilbert rows of any length: chirp-z (Bluestein) row transform -------------------------------------------------
+// A row length n that the time-axis planner rejects is transformed as a circular convolution of length m: the smallest
+// 2^a 3^b 5^c >= 2 n - 1 that build_fk_hostplan(1, m) accepts.  m <= 25 x 10 240 = 256 000, so n <= 128 000.
+constexpr int kHilbertMaxSamples = 128000;
+
+struct RowCztPlan {
+    int n = 0, m = 0;
+    int fused = 0;                    // split rows: middle pass by k_row_mid_fused (tables in its order)
+    FkHostPlan hp;                    // the length-m row plan (t1, t2, rowpl, twiddles, table orders)
+    std::vector<float2> chirp;        // c[t], t < n
+    std::vector<float2> bhat;         // FFT_m(conj c, wrapped) / m in the middle pass's table order
+};
+
+// returns 0, or 1 with err set (n above kHilbertMaxSamples)
+inline int plan_czt_rows(int n, size_t smem_cap, RowCztPlan& rp, std::string& err, int row_fused_default = 1) {
+    if (n < 1 || n > kHilbertMaxSamples) {
+        err = "row length " + std::to_string(n) + " has no mixed-radix split, and chirp-z rows are limited to " +
+              std::to_string(kHilbertMaxSamples) + " samples; crop the record";
+        return 1;
+    }
+    std::string e2;
+    int m = next_5smooth(2 * n - 1);
+    while (build_fk_hostplan(1, m, smem_cap, rp.hp, e2, /*allow_row_dual=*/false, row_fused_default)) {
+        m = next_5smooth(m + 1);
+        if (m > 25 * 10240) { err = "row length " + std::to_string(n) + ": no chirp-z length fits the row engine"; return 1; }
+        rp.hp = FkHostPlan();
+    }
+    const FkHostPlan& hp = rp.hp;
+    rp.n = n; rp.m = m;
+    rp.fused = (hp.t1 > 1 && hp.row_fused) ? 1 : 0;
+    const std::vector<int>& order = rp.fused ? hp.pos2k_row_tab : hp.pos2k_row;
+    std::vector<int> tab2freq((size_t)m);
+    for (int kt1 = 0; kt1 < hp.t1; ++kt1)
+        for (int pos = 0; pos < hp.t2; ++pos) tab2freq[(size_t)kt1 * hp.t2 + pos] = kt1 + hp.t1 * order[pos];
+    czt_tables(n, m, tab2freq, rp.chirp, rp.bhat);
     return 0;
 }
 

@@ -520,8 +520,10 @@ __host__ __device__ inline void body_row_split(float2* __restrict__ w, size_t ld
 // ------------------------------------------------------------------ P3: FFT(T2) -> x table -> IFFT(T2)
 // `tab` is indexed [slot*tab_slot_stride + kt1*T2 + p] in transform (digit-reversed) order;
 // tab_slot_stride = 0 shares one table between all rows (Hilbert weights, template spectra).
+// TabT = float2 (the chirp-z Hilbert rows' kernel spectrum): the table multiplies instead of scaling.
+template <typename TabT>
 __host__ __device__ inline void body_row_mid(const RowParams& rp, float2* __restrict__ w, size_t ldw,
-                                             const float* __restrict__ tab, size_t tab_slot_stride, int kt1, int slot,
+                                             const TabT* __restrict__ tab, size_t tab_slot_stride, int kt1, int slot,
                                              int tid, int nthr, float2* smem) {
     const int n = rp.t2;
     float2* g = w + (size_t)slot * ldw + (size_t)kt1 * n;
@@ -539,8 +541,12 @@ __host__ __device__ inline void body_row_mid(const RowParams& rp, float2* __rest
         D4W_SYNC();
     }
     fft_forward_stages(smem, rp.pl, rp.tw, 1, n, tid, nthr, 0, rp.pl.nstages);
-    const float* m = tab + (size_t)slot * tab_slot_stride + (size_t)kt1 * n;
-    for (int i = tid; i < n; i += nthr) { const float s = m[i]; float2 v = smem[i]; v.x *= s; v.y *= s; smem[i] = v; }
+    const TabT* m = tab + (size_t)slot * tab_slot_stride + (size_t)kt1 * n;
+    if constexpr (std::is_same<TabT, float>::value) {
+        for (int i = tid; i < n; i += nthr) { const float s = m[i]; float2 v = smem[i]; v.x *= s; v.y *= s; smem[i] = v; }
+    } else {
+        for (int i = tid; i < n; i += nthr) smem[i] = cmul(smem[i], m[i]);
+    }
     D4W_SYNC();
     fft_inverse_stages(smem, rp.pl, rp.tw, 1, n, tid, nthr, 0, rp.pl.nstages);
     for (int i = tid; i < n; i += nthr) g[i] = smem[i];
@@ -1009,15 +1015,18 @@ __host__ __device__ inline void row_first_inv(float2* __restrict__ g, const floa
         static_for<R>([&](auto qc) { constexpr int q = decltype(qc)::value; g[n + q * L] = v[q]; });
     }
 }
-template <int R>
-__host__ __device__ inline void row_last_masked(float2* __restrict__ s, const float* __restrict__ tab, int n_total, int tid, int nthr) {
+template <int R, typename TabT>
+__host__ __device__ inline void row_last_masked(float2* __restrict__ s, const TabT* __restrict__ tab, int n_total, int tid, int nthr) {
     const int G = n_total / R;
     for (int j = tid; j < G; j += nthr) {
         float2* base = s + j * R;
         float2 v[R];
         static_for<R>([&](auto qc) { constexpr int q = decltype(qc)::value; v[q] = base[q]; });
         DFT<R, false>::run(v);
-        static_for<R>([&](auto mc) { constexpr int m = decltype(mc)::value; const float c = tab[m * G + j]; v[m].x *= c; v[m].y *= c; });
+        if constexpr (std::is_same<TabT, float>::value)
+            static_for<R>([&](auto mc) { constexpr int m = decltype(mc)::value; const float c = tab[m * G + j]; v[m].x *= c; v[m].y *= c; });
+        else
+            static_for<R>([&](auto mc) { constexpr int m = decltype(mc)::value; v[m] = cmul(v[m], tab[m * G + j]); });
         DFT<R, true>::run(v);
         static_for<R>([&](auto qc) { constexpr int q = decltype(qc)::value; base[q] = v[q]; });
     }
@@ -1031,12 +1040,13 @@ __host__ __device__ inline void row_last_masked(float2* __restrict__ s, const fl
 __host__ __device__ inline bool row_radix_inreg(int r) {
     return r == 2 || r == 3 || r == 4 || r == 5 || r == 6 || r == 8 || r == 10 || r == 12 || r == 15 || r == 16 || r == 20 || r == 25;
 }
+template <typename TabT>
 __host__ __device__ inline void body_row_mid_fused(const RowParams& rp, float2* __restrict__ w, size_t ldw,
-                                                   const float* __restrict__ tab, size_t tab_slot_stride, int kt1, int slot,
+                                                   const TabT* __restrict__ tab, size_t tab_slot_stride, int kt1, int slot,
                                                    int tid, int nthr, float2* smem) {
     const int n = rp.t2, nst = rp.pl.nstages;
     float2* g = w + (size_t)slot * ldw + (size_t)kt1 * n;
-    const float* m = tab + (size_t)slot * tab_slot_stride + (size_t)kt1 * n;
+    const TabT* m = tab + (size_t)slot * tab_slot_stride + (size_t)kt1 * n;
     const int r0 = rp.pl.radix[0], rl = rp.pl.radix[nst - 1];
 #define D4W_CALL(R) row_first_fwd<R>(g, smem, rp.tw, n, tid, nthr);
     D4W_ROW_RADIX_SWITCH(r0, D4W_CALL)

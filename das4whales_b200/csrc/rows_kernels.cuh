@@ -12,6 +12,7 @@
 #include <type_traits>
 #include "fft_smem.cuh"
 #include "fk_kernels.cuh"
+#include "hilbert_czt.cuh"
 
 namespace d4w {
 
@@ -549,16 +550,7 @@ k_xcorr_pfa(XcorrParams xp, const int* __restrict__ tpos, const float* __restric
 }
 
 // ------------------------------------------------------------------ Hilbert envelope / SNR on the T1 x T2 row engine
-// EPI_HILB: the Hilbert transform H(x) itself (dsp.instant_freq needs the phase); EPI_ENVSTD: envelope / std_row
-// (improcess.trace2image, improcess.py:61)
-enum { EPI_ENV = 0, EPI_SNR = 1, EPI_HILB = 2, EPI_ENVSTD = 3 };
-
-__device__ __forceinline__ float hilbert_epilogue(float2 z, int mode, float var) {
-    if (mode == EPI_HILB) return z.y;
-    const float p = z.x * z.x + z.y * z.y;
-    if (mode == EPI_ENVSTD) return sqrtf(p) / sqrtf(var);
-    return mode == EPI_ENV ? sqrtf(p) : 10.0f * log10f(p / var);
-}
+// EPI_* modes and hilbert_epilogue / hilbert_epilogue2: hilbert_czt.cuh (shared with the chirp-z rows)
 
 // forward split reading the REAL row (imag = 0) and writing the complex workspace
 template <int T1>
@@ -605,12 +597,6 @@ k_hsplit_inv(const float2* __restrict__ w, int ns, float* __restrict__ out, int 
 // yields H(a) + i H(b): half the transforms and half the workspace traffic of the analytic-signal route.  The middle
 // pass multiplies by the real table sgn(f)/ns (0 at DC and Nyquist, scipy.signal.hilbert's h - 1); the factor -i is
 // applied here: with u = IFFT(Z sgn), H(a) = Im u and H(b) = -Re u; |hilbert(a)| = sqrt(a^2 + H(a)^2).
-__device__ __forceinline__ float hilbert_epilogue2(float x, float h, int mode, float var) {
-    if (mode == EPI_HILB) return h;
-    const float p = x * x + h * h;
-    if (mode == EPI_ENVSTD) return sqrtf(p) / sqrtf(var);
-    return mode == EPI_ENV ? sqrtf(p) : 10.0f * log10f(p / var);
-}
 template <int T1>
 static __global__ void __launch_bounds__(128)
 k_hsplit_fwd2(const float* __restrict__ x, int nx, int ns, float2* __restrict__ w, int t2len, const float2* __restrict__ twT) {

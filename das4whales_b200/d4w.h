@@ -142,10 +142,14 @@ int d4w_xcorr(d4w_fft_plan* plan, const float* dev_x, int nx, int ns, int valid,
 /* ---- Hilbert envelope |scipy.signal.hilbert(x, axis=1)| (detect.py:192) and
  *      dsp.snr_tr_array(trace, env=True) (dsp.py:975).  mode 0: envelope, 1: 10*log10(env^2/var).
  *      dev_out must not overlap dev_x (long rows are transformed two per complex FFT and dev_x is read again at the end).
- *      d4w_xcorr's dev_tabs are in d4w_fft_plan_table_order. */
+ *      d4w_xcorr's dev_tabs are in d4w_fft_plan_table_order.
+ *      Any ns up to 128 000 is accepted: a length with no T1 x T2 split (a prime factor > 61) is transformed by a chirp-z
+ *      convolution of length czt_m = T1 * T2 ~ 2 ns.  d4w_row_plan_info reports the split and czt_m (0: direct transform);
+ *      d4w_row_workspace_bytes sizes the workspace for nx rows of the chosen route. */
 int d4w_row_plan_create(d4w_row_plan** out, int ns, int device);
 int d4w_row_plan_destroy(d4w_row_plan* plan);
 size_t d4w_row_workspace_bytes(const d4w_row_plan* plan, int nx);
+int d4w_row_plan_info(const d4w_row_plan* plan, int* t1, int* t2, int* czt_m);
 int d4w_hilbert(d4w_row_plan* plan, const float* dev_x, float* dev_out, int nx, void* dev_workspace, int mode,
                 const double* dev_stats, void* stream);
 

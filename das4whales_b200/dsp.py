@@ -333,11 +333,14 @@ CZT_MAX_CHANNELS = 12800
 
 
 def supported_shape(nx, ns):
-    """Largest (nx', ns') <= (nx, ns) the f-k / row FFT planner accepts.  The f-k filter takes any channel count up to
+    """Largest (nx', ns') <= (nx, ns) the f-k filter's planner accepts.  The f-k filter takes any channel count up to
     12 800; above that the channel count must have no prime factor > 61 and one channel column must fit an SM's shared
-    memory (about 28 000 channels).  The time axis is mixed-radix: every prime factor must be <= 61 and it must split as
+    memory (about 28 000 channels).  Its time axis is mixed-radix: every prime factor must be <= 61 and it must split as
     ns = T1 * T2 with T1 <= 25 and T2 <= 10 240.  numpy.fft takes any length; crop (or pad the record before loading) to the
-    suggested shape when `fk_filter_filt` / `envelope` raise ValueError for an unsupported length."""
+    suggested shape when `fk_filter_filt` raises ValueError for an unsupported length.
+    The Hilbert family (`envelope`, `pick_times_env`, `snr_tr_array(env=True)`, `instant_freq`, `trace2image`) is not bound
+    by the time-axis rule: a row length without such a split runs through a chirp-z transform up to
+    rows.HILBERT_MAX_SAMPLES = 128 000 samples."""
     def smooth(n):
         for p in (2, 3, 5, 7, 11, 13, 17, 19, 23, 29, 31, 37, 41, 43, 47, 53, 59, 61):
             while n % p == 0:

@@ -48,12 +48,24 @@ def fft_plan(n, device):
     return _fft_plans[key]
 
 
+# Longest row the Hilbert family takes when the length has no T1 x T2 split: its chirp-z convolution (>= 2 ns - 1 points)
+# must split as T1 x T2 <= 25 x 10 240 (csrc/fk_hostplan.hpp, kHilbertMaxSamples).  Lengths with a split have no limit here.
+HILBERT_MAX_SAMPLES = 128000
+
+
 class _RowPlan:
     def __init__(self, ns, device):
         L = _lib.lib()
         out = _lib.ffi.new("d4w_row_plan**")
         _lib.check(L.d4w_row_plan_create(out, int(ns), int(device)), f"row plan ns={ns}")
         self.ptr, self.ns, self.device = out[0], int(ns), int(device)
+        t1, t2, m = _lib.ffi.new("int*"), _lib.ffi.new("int*"), _lib.ffi.new("int*")
+        _lib.check(L.d4w_row_plan_info(self.ptr, t1, t2, m), "row plan info")
+        self.t1, self.t2, self.czt_m = int(t1[0]), int(t2[0]), int(m[0])     # czt_m = 0: direct transform
+
+    def info(self):
+        """(T1, T2, czt_m): the time split of the transform, and the chirp-z convolution length (0 for a direct plan)"""
+        return self.t1, self.t2, self.czt_m
 
 
 def row_plan(ns, device):
@@ -169,8 +181,9 @@ def _hilbert(x, mode, stats=None):
     out = torch.empty_like(x)
     L = _lib.lib()
     with torch.cuda.device(dev):
-        # rows are independent: chunk so the complex workspace stays bounded (and gridDim.y <= 65535)
-        max_rows = max(1, min(65535, (8 << 30) // (ns * 8)))
+        # rows are independent: chunk so the complex workspace stays bounded (and gridDim.y <= 65535); a workspace row is
+        # ns complex samples on the direct route and czt_m ~ 2 ns on the chirp-z route
+        max_rows = max(1, min(65535, (8 << 30) // max(1, int(L.d4w_row_workspace_bytes(plan.ptr, 1)))))
         wsb = L.d4w_row_workspace_bytes(plan.ptr, min(nx, max_rows))
         ws = torch.empty(int(wsb), dtype=torch.uint8, device=x.device)
         for r0 in range(0, nx, max_rows):
