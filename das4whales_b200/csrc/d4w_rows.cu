@@ -5,23 +5,12 @@
 #include "d4w_common.hpp"
 #include "fk_hostplan.hpp"
 #include "rows_kernels.cuh"
+#include "xcorr_launch.cuh"
 
 using namespace d4w;
 
 // ------------------------------------------------------------------ generic smem FFT plan (xcorr blocks, STFT frames)
-struct d4w_fft_plan {
-    int n = 0, device = 0;
-    size_t smem_cap = 0;
-    FftPlan pl{};
-    std::vector<int> pos2k;
-    std::vector<int> tab2k;      // frequency of each entry of a multiplier table in d4w_xcorr's order
-    int fused = 0;               // k_xcorr_fused usable: >= 2 stages, first and last stage in-register radices
-    float2* d_tw = nullptr;
-    int* d_k2pos = nullptr;
-    int pfa = 0;                 // n == 2520: prime-factor blocks of the matched filter (fft_pfa.cuh)
-    int* d_tpos = nullptr;       // pfa: position of time index i
-    float2* d_wn = nullptr;      // exp(-2 pi i j / n), j < n (sliding-DFT STFT)
-};
+// struct d4w_fft_plan: xcorr_launch.cuh
 
 extern "C" int d4w_fft_plan_create(d4w_fft_plan** out, int n, int device) {
     if (!out) return fail(D4W_ERR_ARG, "d4w_fft_plan_create: null output");
@@ -131,46 +120,7 @@ extern "C" int d4w_xcorr(d4w_fft_plan* p, const float* x, int nx, int ns, int va
     if (valid < 1 || valid > p->n || ntpl < 1) return fail(D4W_ERR_ARG, "d4w_xcorr: bad valid / ntpl");
     const bool normalize = dev_stats != nullptr;
     if (normalize && (!dev_segpre || !dev_mu_over_m)) return fail(D4W_ERR_ARG, "d4w_xcorr: normalisation needs stats, segpre and mu");
-    DeviceGuard guard(p->device);
-    XcorrParams xp{};
-    xp.pl = p->pl; xp.tw = p->d_tw; xp.nb = p->n; xp.valid = valid; xp.ntpl = ntpl; xp.ns = ns;
-    xp.normalize = normalize ? 1 : 0;
-    xp.nseg = (ns + valid - 1) / valid;
-    // dual-lane kernel (four segments per CTA, packed f32x2 butterflies): needs the fused plan shape; 2 CTAs per SM
-    const size_t smem_dual = (size_t)2 * p->n * 16 + (size_t)((valid + 7) / 8) * 16 + (size_t)valid * 8 + 16;
-    if (p->pfa) {
-        D4W_CUDA_TRY(cudaFuncSetAttribute(k_xcorr_pfa, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
-        if (smem_dual > 112 * 1024) return fail(D4W_ERR_UNSUPPORTED, "d4w_xcorr: shared memory");
-        dim3 gridp((xp.nseg + 3) / 4, nx);
-        k_xcorr_pfa<<<gridp, kPfaThreads, smem_dual, (cudaStream_t)stream>>>(xp, p->d_tpos, x, (const float2*)dev_tabs, dev_stats, dev_segpre,
-                                                                    dev_mu_over_m, out, (size_t)nx * ns);
-        D4W_CHECK_LAUNCH("k_xcorr_pfa");
-        return D4W_OK;
-    }
-    bool small_radices = true;
-    for (int st = 0; st < p->pl.nstages; ++st) small_radices = small_radices && xcorr_dual_radix_ok(p->pl.radix[st]);
-    if (p->fused && p->pl.nstages >= 2 && small_radices && smem_dual <= 110 * 1024 && env_int("D4W_XCORR_DUAL", 1)) {
-        D4W_CUDA_TRY(cudaFuncSetAttribute(k_xcorr_dual, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
-        dim3 gridd((xp.nseg + 3) / 4, nx);
-        k_xcorr_dual<<<gridd, 256, smem_dual, (cudaStream_t)stream>>>(xp, x, (const float2*)dev_tabs, dev_stats, dev_segpre, dev_mu_over_m,
-                                                                     out, (size_t)nx * ns);
-        D4W_CHECK_LAUNCH("k_xcorr_dual");
-        return D4W_OK;
-    }
-    const size_t smem = (size_t)3 * p->n * sizeof(float2);
-    if (smem + 1024 > p->smem_cap) return fail(D4W_ERR_UNSUPPORTED, "d4w_xcorr: block length too large for shared memory");
-    dim3 grid((xp.nseg + 1) / 2, nx);
-    if (p->fused) {
-        D4W_CUDA_TRY(cudaFuncSetAttribute(k_xcorr_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cap - 1024));
-        k_xcorr_fused<<<grid, 128, smem, (cudaStream_t)stream>>>(xp, x, (const float2*)dev_tabs, dev_stats, dev_segpre, dev_mu_over_m, out,
-                                                                (size_t)nx * ns);
-    } else {
-        D4W_CUDA_TRY(cudaFuncSetAttribute(k_xcorr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cap - 1024));  // minus its static smem
-        k_xcorr<<<grid, 128, smem, (cudaStream_t)stream>>>(xp, x, (const float2*)dev_tabs, dev_stats, dev_segpre, dev_mu_over_m, out,
-                                                          (size_t)nx * ns);
-    }
-    D4W_CHECK_LAUNCH("k_xcorr");
-    return D4W_OK;
+    return xcorr_launch<false>(p, x, nx, ns, valid, ntpl, dev_tabs, dev_mu_over_m, dev_stats, dev_segpre, nullptr, 0, out, stream);
 }
 
 // ------------------------------------------------------------------ Hilbert envelope / envelope SNR

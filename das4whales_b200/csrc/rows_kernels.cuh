@@ -119,9 +119,29 @@ struct XcorrParams {
     int nb, valid, ntpl, ns, normalize, nseg;
 };
 
+// SAME = true: the centred ("same") correlation of scripts/main_gabordetect.py:245, scipy.signal.correlate(x / max(x), c,
+// 'same'), for templates whose taps are prepended with zeros up to a common lag offset lag0 (d4w_xcorr_same).  The block
+// that produces outputs t .. t + V - 1 reads samples t - lag0 .., zero outside [0, ns), scaled by 1 / rowmax[row]; there is
+// no demeaning and no mu term, and a row whose maximum is not > 0 is all zeros (its CTAs write zeros and return before any
+// transform: the branch is uniform, row = blockIdx.y).  SAME = false ignores rowmax and lag0.
+// sample t of a row in SAME mode (t may be negative)
+__device__ __forceinline__ float xcorr_same_load(const float* __restrict__ r, int t, int ns, float inv) {
+    return (t >= 0 && t < ns) ? r[t] * inv : 0.f;
+}
+// zeros for output samples [a, b) of one row, every template
+__device__ __forceinline__ void xcorr_zero_span(float* __restrict__ out, size_t out_tpl_stride, int ntpl, size_t row_off, int a, int b,
+                                                int tid, int nthr) {
+    for (int t = 0; t < ntpl; ++t) {
+        float* o = out + (size_t)t * out_tpl_stride + row_off;
+        for (int i = a + tid; i < b; i += nthr) o[i] = 0.f;
+    }
+}
+
+template <bool SAME>
 static __global__ void __launch_bounds__(128, 4)
 k_xcorr(XcorrParams xp, const float* __restrict__ x, const float2* __restrict__ tabs, const double* __restrict__ stats,
-        const double* __restrict__ segpre, const double* __restrict__ mu_over_m, float* __restrict__ out, size_t out_tpl_stride) {
+        const double* __restrict__ segpre, const double* __restrict__ mu_over_m, float* __restrict__ out, size_t out_tpl_stride,
+        const float* __restrict__ rowmax, int lag0) {
     extern __shared__ float2 sm[];
     float2* S = sm;                   // spectrum of the segment pair
     float2* B = sm + xp.nb;           // work buffer for the inverse
@@ -134,16 +154,26 @@ k_xcorr(XcorrParams xp, const float* __restrict__ x, const float2* __restrict__ 
     const int ta = seg_a * V, tb = seg_b * V;
     const float* r = x + (size_t)row * ns;
     float mean = 0.f, inv = 1.f;
-    if (xp.normalize) { mean = (float)stats[4 * (size_t)row]; inv = (float)(1.0 / stats[4 * (size_t)row + 1]); }
+    if constexpr (SAME) {
+        const float m = rowmax[row];
+        if (!(m > 0.f)) { xcorr_zero_span(out, out_tpl_stride, xp.ntpl, (size_t)row * ns, ta, min(ns, ta + 2 * V), tid, nthr); return; }
+        inv = 1.f / m;
+    } else {
+        if (xp.normalize) { mean = (float)stats[4 * (size_t)row]; inv = (float)(1.0 / stats[4 * (size_t)row + 1]); }
+    }
     for (int i = tid; i < nb; i += nthr) {
         const int ia = ta + i, ib = tb + i;
-        const float a = (ia < ns) ? (r[ia] - mean) * inv : 0.f;
-        const float b = (ib < ns) ? (r[ib] - mean) * inv : 0.f;
-        S[i] = make_float2(a, b);
+        if constexpr (SAME) {
+            S[i] = make_float2(xcorr_same_load(r, ia - lag0, ns, inv), xcorr_same_load(r, ib - lag0, ns, inv));
+        } else {
+            const float a = (ia < ns) ? (r[ia] - mean) * inv : 0.f;
+            const float b = (ib < ns) ? (r[ib] - mean) * inv : 0.f;
+            S[i] = make_float2(a, b);
+        }
     }
     __syncthreads();
     // exclusive prefix of the first V samples of each segment (only needed for the mu term)
-    if (xp.normalize) {
+    if (!SAME && xp.normalize) {
         const int chunk = (V + nthr - 1) / nthr;
         const int i0 = min(V, tid * chunk), i1 = min(V, i0 + chunk);
         float2 loc = make_float2(0.f, 0.f);
@@ -172,12 +202,12 @@ k_xcorr(XcorrParams xp, const float* __restrict__ x, const float2* __restrict__ 
         for (int i = tid; i < nb; i += nthr) B[i] = cmul(S[i], tab[i]);
         __syncthreads();
         fft_inverse_stages(B, xp.pl, xp.tw, 1, nb, tid, nthr, 0, xp.pl.nstages);
-        const float mu = xp.normalize ? (float)mu_over_m[t] : 0.f;
+        const float mu = (!SAME && xp.normalize) ? (float)mu_over_m[t] : 0.f;
         float* o = out + (size_t)t * out_tpl_stride + (size_t)row * ns;
         for (int i = tid; i < V; i += nthr) {
             const float2 v = B[i];
             float2 p = make_float2(0.f, 0.f);
-            if (xp.normalize) p = P[i];
+            if (!SAME && xp.normalize) p = P[i];
             // out = (sum x~ c - mu * suffix) / m, suffix = -prefix because x~ sums to zero
             if (ta + i < ns) o[ta + i] = v.x + mu * p.x;
             if (tb + i < ns) o[tb + i] = v.y + mu * p.y;
@@ -227,9 +257,11 @@ __device__ __forceinline__ void xcorr_first_inv_out(const float2* __restrict__ B
     }
 }
 
+template <bool SAME>
 static __global__ void __launch_bounds__(128, 4)
 k_xcorr_fused(XcorrParams xp, const float* __restrict__ x, const float2* __restrict__ tabs, const double* __restrict__ stats,
-              const double* __restrict__ segpre, const double* __restrict__ mu_over_m, float* __restrict__ out, size_t out_tpl_stride) {
+              const double* __restrict__ segpre, const double* __restrict__ mu_over_m, float* __restrict__ out, size_t out_tpl_stride,
+              const float* __restrict__ rowmax, int lag0) {
     extern __shared__ float2 sm[];
     float2* S = sm;
     float2* B = sm + xp.nb;
@@ -242,15 +274,25 @@ k_xcorr_fused(XcorrParams xp, const float* __restrict__ x, const float2* __restr
     const int ta = seg_a * V, tb = seg_b * V;
     const float* r = x + (size_t)row * ns;
     float mean = 0.f, inv = 1.f;
-    if (xp.normalize) { mean = (float)stats[4 * (size_t)row]; inv = (float)(1.0 / stats[4 * (size_t)row + 1]); }
+    if constexpr (SAME) {
+        const float m = rowmax[row];
+        if (!(m > 0.f)) { xcorr_zero_span(out, out_tpl_stride, xp.ntpl, (size_t)row * ns, ta, min(ns, ta + 2 * V), tid, nthr); return; }
+        inv = 1.f / m;
+    } else {
+        if (xp.normalize) { mean = (float)stats[4 * (size_t)row]; inv = (float)(1.0 / stats[4 * (size_t)row + 1]); }
+    }
     for (int i = tid; i < nb; i += nthr) {
         const int ia = ta + i, ib = tb + i;
-        const float a = (ia < ns) ? (r[ia] - mean) * inv : 0.f;
-        const float b = (ib < ns) ? (r[ib] - mean) * inv : 0.f;
-        S[i] = make_float2(a, b);
+        if constexpr (SAME) {
+            S[i] = make_float2(xcorr_same_load(r, ia - lag0, ns, inv), xcorr_same_load(r, ib - lag0, ns, inv));
+        } else {
+            const float a = (ia < ns) ? (r[ia] - mean) * inv : 0.f;
+            const float b = (ib < ns) ? (r[ib] - mean) * inv : 0.f;
+            S[i] = make_float2(a, b);
+        }
     }
     __syncthreads();
-    if (xp.normalize) {
+    if (!SAME && xp.normalize) {
         const int chunk = (V + nthr - 1) / nthr;
         const int i0 = min(V, tid * chunk), i1 = min(V, i0 + chunk);
         float2 loc = make_float2(0.f, 0.f);
@@ -282,9 +324,9 @@ k_xcorr_fused(XcorrParams xp, const float* __restrict__ x, const float2* __restr
 #undef D4W_CALL
         __syncthreads();
         fft_inverse_stages(B, xp.pl, xp.tw, 1, nb, tid, nthr, 1, nst - 1);
-        const float mu = xp.normalize ? (float)mu_over_m[t] : 0.f;
+        const float mu = (!SAME && xp.normalize) ? (float)mu_over_m[t] : 0.f;
         float* o = out + (size_t)t * out_tpl_stride + (size_t)row * ns;
-#define D4W_CALL(R) xcorr_first_inv_out<R>(B, P, xp.tw, nb, V, ta, tb, ns, mu, xp.normalize != 0, o, tid, nthr);
+#define D4W_CALL(R) xcorr_first_inv_out<R>(B, P, xp.tw, nb, V, ta, tb, ns, mu, !SAME && xp.normalize != 0, o, tid, nthr);
         D4W_ROW_RADIX_SWITCH(r0, D4W_CALL)
 #undef D4W_CALL
         __syncthreads();
@@ -361,9 +403,11 @@ __device__ __forceinline__ void stage_dispatch_dual_small(cpd* s, const float2* 
 #undef D4W_CALL
 }
 
+template <bool SAME>
 static __global__ void __launch_bounds__(256, 2)
 k_xcorr_dual(XcorrParams xp, const float* __restrict__ x, const float2* __restrict__ tabs, const double* __restrict__ stats,
-             const double* __restrict__ segpre, const double* __restrict__ mu_over_m, float* __restrict__ out, size_t out_tpl_stride) {
+             const double* __restrict__ segpre, const double* __restrict__ mu_over_m, float* __restrict__ out, size_t out_tpl_stride,
+             const float* __restrict__ rowmax, int lag0) {
     extern __shared__ __align__(16) unsigned char smraw[];
     const int ns = xp.ns, nb = xp.nb, V = xp.valid, nst = xp.pl.nstages;
     const int ng = (V + 7) >> 3;                           // prefix groups of 8 samples
@@ -378,17 +422,29 @@ k_xcorr_dual(XcorrParams xp, const float* __restrict__ x, const float2* __restri
     const int t0 = seg0 * V;
     const float* r = x + (size_t)row * ns;
     float mean = 0.f, inv = 1.f;
-    if (xp.normalize) { mean = (float)stats[4 * (size_t)row]; inv = (float)(1.0 / stats[4 * (size_t)row + 1]); }
+    if constexpr (SAME) {
+        const float m = rowmax[row];
+        if (!(m > 0.f)) { xcorr_zero_span(out, out_tpl_stride, xp.ntpl, (size_t)row * ns, t0, min(ns, t0 + 4 * V), tid, nthr); return; }
+        inv = 1.f / m;
+    } else {
+        if (xp.normalize) { mean = (float)stats[4 * (size_t)row]; inv = (float)(1.0 / stats[4 * (size_t)row + 1]); }
+    }
     for (int i = tid; i < nb; i += nthr) {
         const int ia = t0 + i, ib = ia + V, ic = ib + V, id = ic + V;
-        const float a = (ia < ns) ? (r[ia] - mean) * inv : 0.f;
-        const float b = (ib < ns) ? (r[ib] - mean) * inv : 0.f;
-        const float c = (ic < ns) ? (r[ic] - mean) * inv : 0.f;
-        const float d = (id < ns) ? (r[id] - mean) * inv : 0.f;
-        S[i] = dmake(f2x_set(a, c), f2x_set(b, d));
+        if constexpr (SAME) {
+            const float a = xcorr_same_load(r, ia - lag0, ns, inv), b = xcorr_same_load(r, ib - lag0, ns, inv);
+            const float c = xcorr_same_load(r, ic - lag0, ns, inv), d = xcorr_same_load(r, id - lag0, ns, inv);
+            S[i] = dmake(f2x_set(a, c), f2x_set(b, d));
+        } else {
+            const float a = (ia < ns) ? (r[ia] - mean) * inv : 0.f;
+            const float b = (ib < ns) ? (r[ib] - mean) * inv : 0.f;
+            const float c = (ic < ns) ? (r[ic] - mean) * inv : 0.f;
+            const float d = (id < ns) ? (r[id] - mean) * inv : 0.f;
+            S[i] = dmake(f2x_set(a, c), f2x_set(b, d));
+        }
     }
     __syncthreads();
-    if (xp.normalize) {
+    if (!SAME && xp.normalize) {
         // exclusive prefix of the first V samples of each of the four segments: thread -> contiguous run of groups
         const int gpt = (ng + nthr - 1) / nthr;
         const int g0 = min(ng, tid * gpt), g1 = min(ng, g0 + gpt);
@@ -440,9 +496,9 @@ k_xcorr_dual(XcorrParams xp, const float* __restrict__ x, const float2* __restri
             stage_dispatch_dual_small<true>(B, xp.tw, nb, xp.pl.sub[st], xp.pl.radix[st], tid, nthr);
             __syncthreads();
         }
-        const float mu = xp.normalize ? (float)mu_over_m[t] : 0.f;
+        const float mu = (!SAME && xp.normalize) ? (float)mu_over_m[t] : 0.f;
         float* o = out + (size_t)t * out_tpl_stride + (size_t)row * ns;
-#define D4W_CALL(R) xcorrd_first_inv_out<R>(B, Pc, Pf, xp.tw, nb, V, t0, ns, mu, xp.normalize != 0, o, tid, nthr);
+#define D4W_CALL(R) xcorrd_first_inv_out<R>(B, Pc, Pf, xp.tw, nb, V, t0, ns, mu, !SAME && xp.normalize != 0, o, tid, nthr);
         D4W_SMALL_RADIX_SWITCH(r0, D4W_CALL)
 #undef D4W_CALL
         __syncthreads();
@@ -454,10 +510,11 @@ k_xcorr_dual(XcorrParams xp, const float* __restrict__ x, const float2* __restri
 // prefix-summed, scattered to the 4-D positions (S), transformed, and the result is gathered back to time order on the way out
 // so that every global access stays coalesced.  tabs[t][m * 280 + j] belongs to position j * 9 + m (d4w_fft_plan_table_order).
 constexpr int kPfaThreads = 256;      // measured: 256 threads 10.8 ms, 320 threads 11.2 ms (10 000 x 120 000, HF + LF)
+template <bool SAME>
 static __global__ void __launch_bounds__(kPfaThreads, 2)
 k_xcorr_pfa(XcorrParams xp, const int* __restrict__ tpos, const float* __restrict__ x, const float2* __restrict__ tabs,
             const double* __restrict__ stats, const double* __restrict__ segpre, const double* __restrict__ mu_over_m,
-            float* __restrict__ out, size_t out_tpl_stride) {
+            float* __restrict__ out, size_t out_tpl_stride, const float* __restrict__ rowmax, int lag0) {
     extern __shared__ __align__(16) unsigned char smraw[];
     constexpr int nb = kPfaN;
     const int ns = xp.ns, V = xp.valid;
@@ -472,7 +529,13 @@ k_xcorr_pfa(XcorrParams xp, const int* __restrict__ tpos, const float* __restric
     const int t0 = seg0 * V;
     const float* r = x + (size_t)row * ns;
     float mean = 0.f, inv = 1.f;
-    if (xp.normalize) { mean = (float)stats[4 * (size_t)row]; inv = (float)(1.0 / stats[4 * (size_t)row + 1]); }
+    if constexpr (SAME) {
+        const float m = rowmax[row];
+        if (!(m > 0.f)) { xcorr_zero_span(out, out_tpl_stride, xp.ntpl, (size_t)row * ns, t0, min(ns, t0 + 4 * V), tid, nthr); return; }
+        inv = 1.f / m;
+    } else {
+        if (xp.normalize) { mean = (float)stats[4 * (size_t)row]; inv = (float)(1.0 / stats[4 * (size_t)row + 1]); }
+    }
     // load + normalise in time order (B) and, in the same sweep, the prefix sums of the mu term: lanes 8k .. 8k+7 hold one
     // prefix group, so a 3-step segmented shuffle scan gives the in-group exclusive prefix (Pf, fp16) and the group total
     // (parked in Pc, turned into the exclusive prefix over groups below) -- no shared-memory traffic, no bank conflicts
@@ -480,6 +543,11 @@ k_xcorr_pfa(XcorrParams xp, const int* __restrict__ tpos, const float* __restric
         const int i = i0 + tid;
         const bool in = i < nb;
         const int ia = t0 + i, ib = ia + V, ic = ib + V, id = ic + V;
+        if constexpr (SAME) {
+            if (in) B[i] = dmake(f2x_set(xcorr_same_load(r, ia - lag0, ns, inv), xcorr_same_load(r, ic - lag0, ns, inv)),
+                                 f2x_set(xcorr_same_load(r, ib - lag0, ns, inv), xcorr_same_load(r, id - lag0, ns, inv)));
+            continue;                                             // no mu term
+        }
         const float a = (in && ia < ns) ? (r[ia] - mean) * inv : 0.f;
         const float b = (in && ib < ns) ? (r[ib] - mean) * inv : 0.f;
         const float c = (in && ic < ns) ? (r[ic] - mean) * inv : 0.f;
@@ -498,7 +566,7 @@ k_xcorr_pfa(XcorrParams xp, const int* __restrict__ tpos, const float* __restric
         }
     }
     __syncthreads();
-    if (xp.normalize && tid < 32) {
+    if (!SAME && xp.normalize && tid < 32) {
         // exclusive scan of the group totals by one warp, seeded with the row prefix at the start of each segment
         const size_t sp = (size_t)row * xp.nseg + seg0;
         float4 carry;
@@ -528,12 +596,12 @@ k_xcorr_pfa(XcorrParams xp, const int* __restrict__ tpos, const float* __restric
         pfa_last_fused(S, B, tabs + (size_t)t * nb, tid, nthr);
         __syncthreads();
         pfa_inverse_3(B, tid, nthr);
-        const float mu = xp.normalize ? (float)mu_over_m[t] : 0.f;
+        const float mu = (!SAME && xp.normalize) ? (float)mu_over_m[t] : 0.f;
         float* o = out + (size_t)t * out_tpl_stride + (size_t)row * ns;
         for (int i = tid; i < V; i += nthr) {
             const cpd z = B[tpos[i]];
             float va = f2x_lo(z.x), vc = f2x_hi(z.x), vb = f2x_lo(z.y), vd = f2x_hi(z.y);
-            if (xp.normalize) {
+            if (!SAME && xp.normalize) {
                 const float4 c = Pc[i >> 3];
                 const half4 f = Pf[i];
                 const float2 fac = __half22float2(f.ac), fbd = __half22float2(f.bd);

@@ -138,6 +138,15 @@ int d4w_snr(const float* dev_x, float* dev_out, int nx, int ns, const double* de
 int d4w_xcorr(d4w_fft_plan* plan, const float* dev_x, int nx, int ns, int valid, int ntpl, const void* dev_tabs,
               const double* dev_mu_over_m, const double* dev_stats, const double* dev_segpre, float* dev_out,
               void* stream);
+/* ---- "same"-mode matched filter: scipy.signal.correlate(x / max(x), c_t, 'same') of every row with each template
+ *      (scripts/main_gabordetect.py:243-246), on the same overlap-save blocks as d4w_xcorr:
+ *      out[t][row][i] = sum_n x[row][i - lag0 + n] c'_t[n] / rowmax[row], x = 0 outside [0, ns), where c'_t is template t with
+ *      lag0 - floor(L_t / 2) zeros prepended (lag0 = max_t floor(L_t / 2)).  dev_tabs: ntpl x nb complex64 =
+ *      conj(FFT_nb(c'_t)) / nb in d4w_fft_plan_table_order; valid = nb - max_t len(c'_t) + 1.  dev_rowmax: float[nx] from
+ *      d4w_row_max (clamped at 0); rows with !(rowmax > 0) are written as zeros.  1 <= nx <= 65535.
+ *      dev_out: float32 [ntpl][nx][ns]. */
+int d4w_xcorr_same(d4w_fft_plan* plan, const float* dev_x, int nx, int ns, int valid, int lag0, int ntpl, const void* dev_tabs,
+                   const float* dev_rowmax, float* dev_out, void* stream);
 
 /* ---- Hilbert envelope |scipy.signal.hilbert(x, axis=1)| (detect.py:192) and
  *      dsp.snr_tr_array(trace, env=True) (dsp.py:975).  mode 0: envelope, 1: 10*log10(env^2/var).

@@ -106,6 +106,23 @@ def compute_cross_correlograms(data, templates):
     return outs if _is_tensor(data) else [_to_host64(o) for o in outs]
 
 
+def compute_cross_correlogram_same(data, template):
+    """Matched filter of scripts/main_gabordetect.py:238-246 (there is no library function for it): for every channel,
+    `scipy.signal.correlate(row / max(row), template, mode='same')` with the un-padded template (the script's Hann-windowed
+    hyperbolic chirp), no demeaning.  Channels whose maximum is <= 0 -- the ones a Gabor mask zeroes -- come back as zeros
+    (the script skips them and leaves np.empty_like values).  ndarray in -> float64 ndarray out; CUDA tensor in -> float32
+    CUDA tensor out."""
+    return compute_cross_correlograms_same(data, [template])[0]
+
+
+def compute_cross_correlograms_same(data, templates):
+    """compute_cross_correlogram_same for several templates in ONE pass over the data (the HF and LF notes of
+    scripts/main_gabordetect.py:223-246).  Returns a list with one correlogram per template."""
+    xd = _to_device(data)
+    outs = _rows.cross_correlogram_same(xd, [_host1d(t) for t in templates])
+    return outs if _is_tensor(data) else [_to_host64(o) for o in outs]
+
+
 def envelope(corr_m):
     """|hilbert(row)| for every row -- the quantity pick_times_env thresholds (detect.py:192)."""
     y = _rows.envelope(_to_device(corr_m))

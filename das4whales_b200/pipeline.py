@@ -1,6 +1,6 @@
-"""File-level matched-filter detection pipeline on one GPU (BASELINE config 5: one file per GPU).
+"""File-level detection pipelines on one GPU (BASELINE config 5: one file per GPU).
 
-The device-side equivalent of scripts/main_mfdetect.py:42-103 of the reference:
+`MfDetectPipeline` is the device-side equivalent of scripts/main_mfdetect.py:42-103 of the reference:
 
     raw counts (int32, as stored in the HDF5 file)           data_handle.load_das_data / raw2strain   (data_handle.py:157-214)
       -> strain (demean, scale)                               d4w_raw2strain
@@ -11,21 +11,30 @@ The device-side equivalent of scripts/main_mfdetect.py:42-103 of the reference:
       -> Hilbert envelope + prominence peak picking           detect.pick_times_env x 2                (:98-99)
       -> (channel, sample) pick lists                         detect.convert_pick_times                (:102-103)
 
+`GaborDetectPipeline` is the same for scripts/main_gabordetect.py:58-266: the same strain, band-pass and f-k front end,
+then the image-domain Gabor mask (improcess.gabor_detect, :78-169) and the script's own matched filter -- a centred
+("same") correlation of each masked channel divided by its maximum with the un-padded HF / LF notes, channels whose
+maximum is <= 0 skipped (detect.compute_cross_correlograms_same, :223-246) -- before the same threshold and picking (:252-266).
+
 Only the raw counts go up (pinned int32, 4 bytes per sample) and only the picks come down; every intermediate matrix
-stays in HBM.  `MfDetectPipeline.stream(files)` overlaps the H2D copy of file i+1 with the processing of file i.
+stays in HBM.  `stream(files)` overlaps the H2D copy of file i+1 with the processing of file i.
 """
 import numpy as np
 
 from . import detect as _detect
 from . import dsp as _dsp
 from . import fk as _fk
+from . import improcess as _improcess
 from . import rows as _rows
 
 
-class MfDetectPipeline:
-    def __init__(self, nx, ns, selected_channels, dx, fs, scale_factor, device=None, fmin=14., fmax=30.,
-                 mask_speeds=(1350., 1450., 3300, 3450), hf=(17.8, 28.8, 0.68), lf=(14.7, 21.8, 0.78), thres_frac=0.5,
-                 prune_eps=0.0, bandpass=True):
+class _FilePipeline:
+    """Shared part of the file pipelines: strain -> band-pass -> hybrid_ninf f-k filter on the device, the
+    threshold-and-pick tail, and the double-buffered upload of `stream`.  Subclasses set self.templates and implement
+    _correlograms(y) -> (list of [nx, ns] correlograms, extra results)."""
+
+    def __init__(self, nx, ns, selected_channels, dx, fs, scale_factor, device, fmin, fmax, mask_speeds, thres_frac,
+                 prune_eps, bandpass):
         import scipy.signal as sp
         torch = _fk._torch()
         self.torch = torch
@@ -38,34 +47,29 @@ class MfDetectPipeline:
             self.mask = _dsp.hybrid_ninf_filter_design((nx, ns), selected_channels, dx, fs, *mask_speeds, fmin=fmin, fmax=fmax)
             self.fk = _fk.FkFilter(self.mask, device=self.device, eps=prune_eps)
         self.sos = sp.butter(8, [fmin / (fs / 2), fmax / (fs / 2)], "bp", output="sos")          # dsp.bp_filt (dsp.py:878)
-        time = np.arange(ns) / fs
-        self.templates = [_detect.gen_template_fincall(time, fs, *hf), _detect.gen_template_fincall(time, fs, *lf)]
         self._raw = [None, None]
         self._h2d = None
 
     # ---- device side -------------------------------------------------------------------------------------------------
-    def process_device(self, raw, with_snr=False):
-        """raw: int32 (or float32) CUDA tensor [nx, ns] of interrogator counts.  Returns a dict of DEVICE results:
-        picks_hf / picks_lf = (offsets int32 [nx + 1], idx int32 [n]) , maxv (0-dim tensor), optionally snr_hf / snr_lf."""
+    def _filtered(self, raw):
+        x = _rows.raw2strain(raw, self.scale_factor)
+        if self.bandpass:
+            x = _rows.sosfiltfilt(self.sos, x, padlen=3 * 17)
+        return self.fk(x, out=x)
+
+    def _pick(self, corr, with_snr):
         torch = self.torch
-        with torch.cuda.device(self.device):
-            x = _rows.raw2strain(raw, self.scale_factor)
-            if self.bandpass:
-                x = _rows.sosfiltfilt(self.sos, x, padlen=3 * 17)
-            y = self.fk(x, out=x)
-            corr = _rows.cross_correlogram_chunked(y, self.templates, normalize=True)
-            del x, y
-            rmax = torch.stack([_rows.row_max(c) for c in corr])                     # [2, nx]
-            maxv = _rows.row_max(rmax.reshape(1, -1))[0]
-            thres = self.thres_frac * float(maxv.item())                             # main_mfdetect.py:95 (one scalar D2H)
-            out = {"maxv": maxv, "threshold": thres}
-            for name, c, thr in (("hf", corr[0], thres * 0.9), ("lf", corr[1], thres)):
-                env = _rows.envelope(c)
-                out["picks_" + name] = _rows.find_peaks_device(env, thr)
-                del env
-                if with_snr:
-                    out["snr_" + name] = _rows.snr(c, env=True)
-            return out
+        rmax = torch.stack([_rows.row_max(c) for c in corr])                     # [2, nx]
+        maxv = _rows.row_max(rmax.reshape(1, -1))[0]
+        thres = self.thres_frac * float(maxv.item())                             # main_mfdetect.py:95 (one scalar D2H)
+        out = {"maxv": maxv, "threshold": thres}
+        for name, c, thr in (("hf", corr[0], thres * 0.9), ("lf", corr[1], thres)):
+            env = _rows.envelope(c)
+            out["picks_" + name] = _rows.find_peaks_device(env, thr)
+            del env
+            if with_snr:
+                out["snr_" + name] = _rows.snr(c, env=True)
+        return out
 
     @staticmethod
     def picks_to_host(picks):
@@ -126,9 +130,72 @@ class MfDetectPipeline:
             i += 1
 
 
+class MfDetectPipeline(_FilePipeline):
+    def __init__(self, nx, ns, selected_channels, dx, fs, scale_factor, device=None, fmin=14., fmax=30.,
+                 mask_speeds=(1350., 1450., 3300, 3450), hf=(17.8, 28.8, 0.68), lf=(14.7, 21.8, 0.78), thres_frac=0.5,
+                 prune_eps=0.0, bandpass=True):
+        super().__init__(nx, ns, selected_channels, dx, fs, scale_factor, device, fmin, fmax, mask_speeds, thres_frac,
+                         prune_eps, bandpass)
+        time = np.arange(ns) / fs
+        self.templates = [_detect.gen_template_fincall(time, fs, *hf), _detect.gen_template_fincall(time, fs, *lf)]
+
+    def process_device(self, raw, with_snr=False):
+        """raw: int32 (or float32) CUDA tensor [nx, ns] of interrogator counts.  Returns a dict of DEVICE results:
+        picks_hf / picks_lf = (offsets int32 [nx + 1], idx int32 [n]) , maxv (0-dim tensor), optionally snr_hf / snr_lf."""
+        torch = self.torch
+        with torch.cuda.device(self.device):
+            y = self._filtered(raw)
+            corr = _rows.cross_correlogram_chunked(y, self.templates, normalize=True)
+            del y
+            return self._pick(corr, with_snr)
+
+
+class GaborDetectPipeline(_FilePipeline):
+    """scripts/main_gabordetect.py:58-266 on the device; the script's values are the defaults.  Same interface as
+    MfDetectPipeline (process_device / process_file / stream)."""
+
+    def __init__(self, nx, ns, selected_channels, dx, fs, scale_factor, device=None, fmin=14., fmax=30.,
+                 mask_speeds=(1350., 1450., 3300, 3450), hf=(17.8, 28.8, 0.68), lf=(14.7, 21.8, 0.78), thres_frac=0.5,
+                 c0=1500., bin_factor=10, threshold=9100., threshold2=150., prune_eps=0.0, bandpass=True):
+        super().__init__(nx, ns, selected_channels, dx, fs, scale_factor, device, fmin, fmax, mask_speeds, thres_frac,
+                         prune_eps, bandpass)
+        self.dx, self.selected_channels = float(dx), list(selected_channels)
+        self.c0, self.bin_factor = float(c0), int(bin_factor)
+        self.threshold, self.threshold2 = float(threshold), float(threshold2)
+        notes = []
+        for fmin_, fmax_, dur in (hf, lf):                                    # main_gabordetect.py:223-227
+            c = _detect.gen_hyperbolic_chirp(fmin_, fmax_, dur, fs)
+            notes.append(np.hanning(len(c)) * c)
+        self.templates = notes
+
+    def process_device(self, raw, with_snr=False, with_intermediates=False):
+        """raw: int32 (or float32) CUDA tensor [nx, ns] of interrogator counts.  Returns a dict of DEVICE results:
+        picks_hf / picks_lf = (offsets int32 [nx + 1], idx int32 [n]), maxv (0-dim tensor), optionally snr_hf / snr_lf and,
+        with_intermediates, the masked trace ("masked") and the HF / LF correlograms ("corr")."""
+        torch = self.torch
+        with torch.cuda.device(self.device):
+            y = self._filtered(raw)
+            masked = _improcess.gabor_detect(y, self.fs, self.dx, self.selected_channels, c0=self.c0,
+                                             bin_factor=self.bin_factor, threshold=self.threshold, threshold2=self.threshold2)
+            del y
+            corr = _rows.cross_correlogram_same(masked, self.templates)
+            out = self._pick(corr, with_snr)
+            if with_intermediates:
+                out["masked"], out["corr"] = masked, corr
+            return out
+
+
 def process_file(raw, metadata, selected_channels, **kw):
     """Convenience wrapper: raw [nx, ns] counts + the reference's metadata dict (data_handle.get_acquisition_parameters:
     fs, dx, scale_factor) -> picks of the HF and LF fin-whale notes."""
     nx, ns = raw.shape
     pipe = MfDetectPipeline(nx, ns, selected_channels, metadata["dx"], metadata["fs"], metadata["scale_factor"], **kw)
+    return pipe.process_file(raw)
+
+
+def process_file_gabor(raw, metadata, selected_channels, **kw):
+    """Convenience wrapper of GaborDetectPipeline: raw [nx, ns] counts + the reference's metadata dict (fs, dx,
+    scale_factor) -> picks of the HF and LF fin-whale notes of scripts/main_gabordetect.py."""
+    nx, ns = raw.shape
+    pipe = GaborDetectPipeline(nx, ns, selected_channels, metadata["dx"], metadata["fs"], metadata["scale_factor"], **kw)
     return pipe.process_file(raw)

@@ -158,18 +158,68 @@ def cross_correlogram(x, templates, normalize=True):
 _MAX_ROWS = 65535       # gridDim.y limit of the row kernels
 
 
-def cross_correlogram_chunked(x, templates, normalize=True):
-    """cross_correlogram for any number of rows (the kernels take <= 65535 rows per launch)."""
+def _row_chunked(corr, x, ntpl):
+    """corr(rows) -> ntpl float32 tensors [len(rows), ns], for any number of rows: corr is called on slices of <= 65535 rows
+    (the kernels' launch limit) and the parts are copied into whole-matrix outputs."""
     torch = _torch()
     nx = x.shape[0]
     if nx <= _MAX_ROWS:
-        return cross_correlogram(x, templates, normalize)
-    outs = [torch.empty_like(x) for _ in templates]
+        return corr(slice(0, nx))
+    outs = [torch.empty_like(x) for _ in range(ntpl)]
     for r0 in range(0, nx, _MAX_ROWS):
-        part = cross_correlogram(x[r0:r0 + _MAX_ROWS], templates, normalize)
+        part = corr(slice(r0, r0 + _MAX_ROWS))
         for o, p in zip(outs, part):
             o[r0:r0 + _MAX_ROWS] = p
     return outs
+
+
+def cross_correlogram_chunked(x, templates, normalize=True):
+    """cross_correlogram for any number of rows (the kernels take <= 65535 rows per launch)."""
+    return _row_chunked(lambda rs: cross_correlogram(x[rs], templates, normalize), x, len(templates))
+
+
+def same_mode_layout(templates, ns):
+    """Host side of the "same"-mode correlation (d4w_xcorr_same), pure NumPy.
+    templates: 1-D tap arrays c_t (un-padded, any lengths).  Template t gets D - floor(L_t / 2) zeros prepended, D = max_t
+    floor(L_t / 2), so every template has the same lag offset lag0 = D and one forward transform per block serves all of
+    them.  Returns (taps, lag0, nb, valid, spec): the prepended taps, the block length (_pick_block of the longest prepended
+    template), the outputs kept per block and spec[t] = conj(FFT_nb(taps[t])) / nb in natural frequency order."""
+    cs = [np.asarray(c, dtype=np.float64).ravel() for c in templates]
+    if not cs or any(len(c) == 0 for c in cs):
+        raise ValueError("same-mode correlation needs at least one non-empty template")
+    lag0 = max(len(c) // 2 for c in cs)
+    taps = [np.concatenate((np.zeros(lag0 - len(c) // 2), c)) for c in cs]
+    lmax = max(len(c) for c in taps)
+    nb = _pick_block(lmax, ns)
+    valid = nb - lmax + 1
+    spec = np.stack([np.conj(np.fft.fft(c, nb)) / nb for c in taps])
+    return taps, lag0, nb, valid, spec
+
+
+def cross_correlogram_same(x, templates):
+    """scipy.signal.correlate(row / max(row), c, mode='same') of every row with each template, in one pass over the data
+    (scripts/main_gabordetect.py:243-246): un-padded templates, no demeaning; a row whose maximum is <= 0 is all zeros (the
+    script skips it).  templates: list of 1-D tap arrays (up to 2 500 taps).  Any number of rows.
+    Returns a list of float32 CUDA tensors [nx, ns]."""
+    torch = _torch()
+    dev = _check_input(x)
+    nx, ns = x.shape
+    _, lag0, nb, valid, spec = same_mode_layout(templates, ns)
+    plan = fft_plan(nb, dev)
+    tabs = np.ascontiguousarray(spec[:, plan.tab2freq], dtype=np.complex64)
+    ntpl = len(templates)
+    with torch.cuda.device(dev):
+        tabs_d = torch.from_numpy(tabs.view(np.float32).reshape(ntpl, nb, 2)).to(x.device)
+        rowmax = row_max(x)                                   # clamped at 0: "> 0" is the script's test, the value its max
+
+        def corr(rs):
+            xs = x[rs]
+            out = torch.empty((ntpl,) + tuple(xs.shape), dtype=torch.float32, device=x.device)
+            _lib.check(_lib.lib().d4w_xcorr_same(plan.ptr, _lib.ptr(xs, "float*"), xs.shape[0], ns, valid, lag0, ntpl,
+                                                 _lib.ptr(tabs_d), _lib.ptr(rowmax[rs], "float*"), _lib.ptr(out, "float*"),
+                                                 _lib.stream_ptr()), "xcorr_same")
+            return [out[i] for i in range(ntpl)]
+        return _row_chunked(corr, x, ntpl)
 
 
 # ------------------------------------------------------------------------------ Hilbert envelope / SNR
