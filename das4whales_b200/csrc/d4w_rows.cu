@@ -502,13 +502,17 @@ extern "C" int d4w_row_fft_mag(d4w_fft_plan* p, const float* x, int nx, size_t l
 }
 
 // ------------------------------------------------------------------ medians / maxima / spectrogram correlation
-extern "C" int d4w_row_median(const float* x, int nrows, size_t n, float* med, void* stream) {
-    if (!x || !med || nrows < 1 || n < 1) return fail(D4W_ERR_ARG, "d4w_row_median: bad argument");
+extern "C" int d4w_row_median_ld(const float* x, int nrows, size_t n, size_t ld, float* med, void* stream) {
+    if (!x || !med || nrows < 1 || n < 1 || ld < n) return fail(D4W_ERR_ARG, "d4w_row_median: bad argument");
     const size_t smem = (size_t)kMedCap * sizeof(float);
     D4W_CUDA_TRY(cudaFuncSetAttribute(k_row_median, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_row_median<<<nrows, kMedThreads, smem, (cudaStream_t)stream>>>(x, n, med);
+    k_row_median<<<nrows, kMedThreads, smem, (cudaStream_t)stream>>>(x, n, ld, med);
     D4W_CHECK_LAUNCH("k_row_median");
     return D4W_OK;
+}
+
+extern "C" int d4w_row_median(const float* x, int nrows, size_t n, float* med, void* stream) {
+    return d4w_row_median_ld(x, nrows, n, n, med, stream);
 }
 
 extern "C" int d4w_row_max(const float* x, int nrows, size_t n, float* mx, void* stream) {
@@ -518,29 +522,104 @@ extern "C" int d4w_row_max(const float* x, int nrows, size_t n, float* mx, void*
     return D4W_OK;
 }
 
-extern "C" int d4w_speccorr(const float* S, int nx, int nf, int nt, const float* K, int kw, const float* med, float* out,
-                            void* stream) {
-    if (!S || !K || !med || !out || nx < 1 || nf < 1 || nt < 1 || kw < 1) return fail(D4W_ERR_ARG, "d4w_speccorr: bad argument");
-    if (nx > 65535) return fail(D4W_ERR_UNSUPPORTED, "d4w_speccorr: more than 65535 rows per call");
-    {
-        const int kwp = (kw + 3) & ~3;
-        const size_t smem4 = ((size_t)nf * kwp + (size_t)nf * (kScTile + kwp)) * sizeof(float);
-        if (env_int("D4W_SPECCORR4", 1) && smem4 <= 110 * 1024) {
-            D4W_CUDA_TRY(cudaFuncSetAttribute(k_speccorr4, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem4));
-            dim3 grid4((nt + kScTile - 1) / kScTile, nx);
-            k_speccorr4<<<grid4, kScThreads, smem4, (cudaStream_t)stream>>>(S, nf, nt, K, kw, kwp, med, out);
-            D4W_CHECK_LAUNCH("k_speccorr4");
-            return D4W_OK;
-        }
+// One spectrogram kernel of d4w_speccorr_multi: its rows are S[:, f0 : f0 + nf, :].
+struct SpecKernel { const float* K; const float* med; float* out; int f0, nf, kw; };
+
+// k_speccorr4 parameters for kernels ks[0 .. nk-1] sharing one staged tile; returns the dynamic shared memory it needs
+static size_t speccorr4_set(const SpecKernel* ks, int nk, int nfs, SpecCorrSet& set) {
+    set = SpecCorrSet{};
+    set.nk = nk; set.nfs = nfs;
+    int c0 = 0, fs0 = nfs, fs1 = 0;
+    for (int k = 0; k < nk; ++k) {
+        c0 = std::max(c0, ks[k].kw / 2);
+        fs0 = std::min(fs0, ks[k].f0);
+        fs1 = std::max(fs1, ks[k].f0 + ks[k].nf);
     }
-    const int tile = 256;
+    int kwp = 4, nsk = 0;
+    for (int k = 0; k < nk; ++k) {
+        set.K[k] = ks[k].K; set.med[k] = ks[k].med; set.out[k] = ks[k].out;
+        set.f0[k] = ks[k].f0 - fs0; set.nf[k] = ks[k].nf; set.kw[k] = ks[k].kw;
+        set.pad[k] = c0 - ks[k].kw / 2;
+        kwp = std::max(kwp, (set.pad[k] + ks[k].kw + 3) & ~3);
+        nsk += ks[k].nf;
+    }
+    set.fs0 = fs0; set.nst = fs1 - fs0; set.c0 = c0; set.kwp = kwp;
+    return ((size_t)nsk * kwp + (size_t)set.nst * (kScTile + kwp)) * sizeof(float);
+}
+
+static int launch_speccorr4(const float* S, int nx, int nt, const SpecCorrSet& set, size_t smem, cudaStream_t st) {
+    D4W_CUDA_TRY(cudaFuncSetAttribute(k_speccorr4, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dim3 grid4((nt + kScTile - 1) / kScTile, nx);
+    k_speccorr4<<<grid4, kScThreads, smem, st>>>(S, nt, set);
+    D4W_CHECK_LAUNCH("k_speccorr4");
+    return D4W_OK;
+}
+
+// Untiled kernel for one spectrogram kernel too wide for k_speccorr4.  k_speccorr reads [nx][nf][nt]: a band of a wider
+// spectrogram (nfs > nf rows) is first copied to a dense stream-ordered scratch matrix.
+static int launch_speccorr_untiled(const float* S, int nx, int nfs, int nt, const SpecKernel& kk, cudaStream_t st) {
+    const int tile = 256, nf = kk.nf, kw = kk.kw;
     const size_t smem = ((size_t)nf * kw + (size_t)nf * (tile + kw)) * sizeof(float);
     if (smem > 200 * 1024) return fail(D4W_ERR_UNSUPPORTED, "d4w_speccorr: kernel too large for shared memory");
     D4W_CUDA_TRY(cudaFuncSetAttribute(k_speccorr, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     dim3 grid((nt + tile - 1) / tile, nx);
-    k_speccorr<<<grid, tile, smem, (cudaStream_t)stream>>>(S, nf, nt, K, kw, med, out);
+    if (nfs == nf) {
+        k_speccorr<<<grid, tile, smem, st>>>(S, nf, nt, kk.K, kw, kk.med, kk.out);
+        D4W_CHECK_LAUNCH("k_speccorr");
+        return D4W_OK;
+    }
+    const size_t band = (size_t)nf * nt * sizeof(float);
+    float* tmp = nullptr;
+    D4W_CUDA_TRY(cudaMallocAsync((void**)&tmp, band * nx, st));
+    cudaError_t e = cudaMemcpy2DAsync(tmp, band, S + (size_t)kk.f0 * nt, (size_t)nfs * nt * sizeof(float), band, nx,
+                                      cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) {
+        k_speccorr<<<grid, tile, smem, st>>>(tmp, nf, nt, kk.K, kw, kk.med, kk.out);
+        e = cudaGetLastError();
+    }
+    const cudaError_t ef = cudaFreeAsync(tmp, st);
+    D4W_CUDA_TRY(e);
+    D4W_CUDA_TRY(ef);
     D4W_CHECK_LAUNCH("k_speccorr");
     return D4W_OK;
+}
+
+// All kernels in one k_speccorr4 pass when their tile fits; otherwise one pass per kernel, tiled or untiled.
+static int speccorr_kernels(const float* S, int nx, int nfs, int nt, const SpecKernel* ks, int nk, cudaStream_t st) {
+    const bool tiled = env_int("D4W_SPECCORR4", 1) != 0;
+    SpecCorrSet set;
+    size_t smem = speccorr4_set(ks, nk, nfs, set);
+    if (tiled && smem <= 110 * 1024) return launch_speccorr4(S, nx, nt, set, smem, st);
+    for (int k = 0; k < nk; ++k) {
+        smem = speccorr4_set(ks + k, 1, nfs, set);
+        const int rc = (tiled && smem <= 110 * 1024) ? launch_speccorr4(S, nx, nt, set, smem, st)
+                                                     : launch_speccorr_untiled(S, nx, nfs, nt, ks[k], st);
+        if (rc != D4W_OK) return rc;
+    }
+    return D4W_OK;
+}
+
+extern "C" int d4w_speccorr(const float* S, int nx, int nf, int nt, const float* K, int kw, const float* med, float* out,
+                            void* stream) {
+    if (!S || !K || !med || !out || nx < 1 || nf < 1 || nt < 1 || kw < 1) return fail(D4W_ERR_ARG, "d4w_speccorr: bad argument");
+    if (nx > 65535) return fail(D4W_ERR_UNSUPPORTED, "d4w_speccorr: more than 65535 rows per call");
+    const SpecKernel kk{K, med, out, 0, nf, kw};
+    return speccorr_kernels(S, nx, nf, nt, &kk, 1, (cudaStream_t)stream);
+}
+
+extern "C" int d4w_speccorr_multi(const float* S, int nx, int nf, int nt, int nk, const int* f0, const int* nfk,
+                                  const float* const* K, const int* kw, const float* const* med, float* const* out,
+                                  void* stream) {
+    if (!S || !f0 || !nfk || !K || !kw || !med || !out || nx < 1 || nf < 1 || nt < 1 || nk < 1 || nk > kScMaxKernels)
+        return fail(D4W_ERR_ARG, "d4w_speccorr_multi: bad argument");
+    SpecKernel ks[kScMaxKernels];
+    for (int k = 0; k < nk; ++k) {
+        if (!K[k] || !med[k] || !out[k] || kw[k] < 1 || nfk[k] < 1 || f0[k] < 0 || f0[k] + nfk[k] > nf)
+            return fail(D4W_ERR_ARG, "d4w_speccorr_multi: bad kernel");
+        ks[k] = SpecKernel{K[k], med[k], out[k], f0[k], nfk[k], kw[k]};
+    }
+    if (nx > 65535) return fail(D4W_ERR_UNSUPPORTED, "d4w_speccorr_multi: more than 65535 rows per call");
+    return speccorr_kernels(S, nx, nf, nt, ks, nk, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------- peak picking

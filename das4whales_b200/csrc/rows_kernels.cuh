@@ -1131,15 +1131,16 @@ __device__ __forceinline__ unsigned int select_rank(const float* __restrict__ r,
     return prefix;
 }
 
+// row r is the n values from x + r * ld (ld >= n): ld = n for a dense matrix, ld > n for a band of rows of a spectrogram
 static __global__ void __launch_bounds__(kMedThreads)
-k_row_median(const float* __restrict__ x, size_t n, float* __restrict__ med) {
+k_row_median(const float* __restrict__ x, size_t n, size_t ld, float* __restrict__ med) {
     extern __shared__ __align__(16) float mbuf[];                // kMedCap floats: samples, then the bracket's contents
     __shared__ unsigned int hist[2048];
     __shared__ unsigned int s_cnt;
     __shared__ unsigned long long s_below[kMedThreads / 32];
     __shared__ float s_lohi[2];
     const int tid = threadIdx.x, lane = tid & 31;
-    const float* r = x + (size_t)blockIdx.x * n;
+    const float* r = x + (size_t)blockIdx.x * ld;
     const size_t rk_hi = n / 2, rk_lo = (n & 1) ? n / 2 : n / 2 - 1;
     const float* src = r;                                        // where the final select runs
     size_t cnt = n, below = 0;
@@ -1249,29 +1250,46 @@ k_speccorr(const float* __restrict__ S, int nf, int nt, const float* __restrict_
 
 // Register-tiled version (default): four consecutive outputs per thread, the time window slides through two float4
 // registers and the kernel row arrives as broadcast float4 -- 2 shared loads per 16 FMAs instead of 2 per FMA.
-// Shared layout: sk [nf][kwp] (kernel rows zero-padded to kwp = multiple of 4), st [nf][w], w = 4 * threads + kwp.
-constexpr int kScThreads = 128, kScTile = 4 * kScThreads;
+// Several kernels share one staged tile: S holds nfs frequency rows per channel, the rows fs0 .. fs0 + nst - 1 (the union
+// of the kernels' bands) are staged once, and kernel k reads its nf[k] rows from staged row f0[k].  Every kernel gets
+// pad[k] = c0 - kw[k] / 2 leading zeros up to the common centre c0 = max kw / 2, so all of them read the same window
+// t - c0 ..; a zero product leaves the fp32 sum unchanged and each kernel keeps its f-ascending, j-ascending order, so
+// every output is bit-equal to a one-kernel launch (and to k_speccorr).
+// Shared layout: sk_k [nf[k]][kwp] for each k (padded kernel rows, kwp = multiple of 4), st [nst][w], w = 4 * threads + kwp.
+constexpr int kScThreads = 128, kScTile = 4 * kScThreads, kScMaxKernels = 8;
+
+struct SpecCorrSet {
+    const float* K[kScMaxKernels];            // [nf][kw] each
+    const float* med[kScMaxKernels];          // [nx] each
+    float* out[kScMaxKernels];                // [nx][nt] each
+    int f0[kScMaxKernels], nf[kScMaxKernels], kw[kScMaxKernels], pad[kScMaxKernels];
+    int nk, nfs, fs0, nst, c0, kwp;
+};
 
 static __global__ void __launch_bounds__(kScThreads)
-k_speccorr4(const float* __restrict__ S, int nf, int nt, const float* __restrict__ K, int kw, int kwp,
-            const float* __restrict__ med, float* __restrict__ out) {
+k_speccorr4(const float* __restrict__ S, int nt, const __grid_constant__ SpecCorrSet set) {
     extern __shared__ __align__(16) float sh4[];
+    const int kwp = set.kwp, nst = set.nst, c0 = set.c0;
     const int w = kScTile + kwp;
-    float* sk = sh4;                          // [nf][kwp]
-    float* st = sh4 + nf * kwp;               // [nf][w]
     const int tid = threadIdx.x;
     const size_t row = blockIdx.y;
     const int t0 = blockIdx.x * kScTile;
-    const int c0 = kw / 2;
-    for (int i = tid; i < nf * kwp; i += kScThreads) {
-        const int f = i / kwp, j = i - f * kwp;
-        sk[i] = j < kw ? K[f * kw + j] : 0.f;
+    float* st = sh4;                                             // [nst][w] after the kernels
+#pragma unroll 1
+    for (int k = 0; k < set.nk; ++k) {
+        const float* K = set.K[k];
+        const int kw = set.kw[k], pad = set.pad[k], n = set.nf[k] * kwp;
+        for (int i = tid; i < n; i += kScThreads) {
+            const int f = i / kwp, j = i - f * kwp - pad;
+            st[i] = (j >= 0 && j < kw) ? K[f * kw + j] : 0.f;
+        }
+        st += n;
     }
-    const float* Sr = S + row * (size_t)nf * nt;
-    const int fq = (nf + 3) >> 2;                                // frequency rows per staging group
+    const float* Sr = S + row * (size_t)set.nfs * nt + (size_t)set.fs0 * nt;
+    const int fq = (nst + 3) >> 2;                               // frequency rows per staging group
 #pragma unroll 1
     for (int gq = 0; gq < 4; ++gq) {
-        const int f0 = gq * fq, f1 = min(nf, f0 + fq);
+        const int f0 = gq * fq, f1 = min(nst, f0 + fq);
         for (int j = tid; j < w; j += kScThreads) {              // column first: bounds and addresses once per column
             const int t = t0 - c0 + j;
             float* dst = st + f0 * w + j;
@@ -1286,40 +1304,49 @@ k_speccorr4(const float* __restrict__ S, int nf, int nt, const float* __restrict
         }
         cp_async_commit();
     }
-    float acc[4] = {0.f, 0.f, 0.f, 0.f};
     const int nq = kwp >> 2;
-    auto mac16 = [&](const float4& lo, const float4& hi, const float4& k) {
-        const float win[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-        const float kk[4] = {k.x, k.y, k.z, k.w};
+    const float* sk = sh4;
+#pragma unroll 1
+    for (int k = 0; k < set.nk; ++k) {                           // kernel 0 overlaps the staging; the others find it landed
+        float acc[4] = {0.f, 0.f, 0.f, 0.f};
+        auto mac16 = [&](const float4& lo, const float4& hi, const float4& kv) {
+            const float win[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+            const float kk[4] = {kv.x, kv.y, kv.z, kv.w};
 #pragma unroll
-        for (int jj = 0; jj < 4; ++jj)
+            for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
-            for (int oo = 0; oo < 4; ++oo) acc[oo] = fmaf(win[jj + oo], kk[jj], acc[oo]);
-    };
+                for (int oo = 0; oo < 4; ++oo) acc[oo] = fmaf(win[jj + oo], kk[jj], acc[oo]);
+        };
+        const int fa = set.f0[k], fb = fa + set.nf[k];
 #pragma unroll 1                                             // one copy of the FMA block: unrolled four times it missed the i-cache
-    for (int gq = 0; gq < 4; ++gq) {
-        if (gq == 0) cp_async_wait_group<3>(); else if (gq == 1) cp_async_wait_group<2>();
-        else if (gq == 2) cp_async_wait_group<1>(); else cp_async_wait_group<0>();
-        __syncthreads();
-#pragma unroll 1
-        for (int f = gq * fq; f < min(nf, (gq + 1) * fq); ++f) {
-            const float4* a = reinterpret_cast<const float4*>(st + f * w) + tid;
-            const float4* b = reinterpret_cast<const float4*>(sk + f * kwp);
-            float4 c0v = a[0], c1v;
-            int q = 0;
-#pragma unroll 1
-            for (; q + 1 < nq; q += 2) {                         // the window ping-pongs between two registers: no moves
-                c1v = a[q + 1]; mac16(c0v, c1v, b[q]);
-                c0v = a[q + 2]; mac16(c1v, c0v, b[q + 1]);
+        for (int gq = 0; gq < 4; ++gq) {
+            if (k == 0) {
+                if (gq == 0) cp_async_wait_group<3>(); else if (gq == 1) cp_async_wait_group<2>();
+                else if (gq == 2) cp_async_wait_group<1>(); else cp_async_wait_group<0>();
+                __syncthreads();
             }
-            if (q < nq) { c1v = a[q + 1]; mac16(c0v, c1v, b[q]); }
+#pragma unroll 1
+            for (int f = max(fa, gq * fq); f < min(fb, (gq + 1) * fq); ++f) {
+                const float4* a = reinterpret_cast<const float4*>(st + f * w) + tid;
+                const float4* b = reinterpret_cast<const float4*>(sk + (f - fa) * kwp);
+                float4 c0v = a[0], c1v;
+                int q = 0;
+#pragma unroll 1
+                for (; q + 1 < nq; q += 2) {                     // the window ping-pongs between two registers: no moves
+                    c1v = a[q + 1]; mac16(c0v, c1v, b[q]);
+                    c0v = a[q + 2]; mac16(c1v, c0v, b[q + 1]);
+                }
+                if (q < nq) { c1v = a[q + 1]; mac16(c0v, c1v, b[q]); }
+            }
         }
-    }
-    const float den = med[row] * (float)kw;             // same expression as the untiled kernel: identical rounding
+        const float den = set.med[k][row] * (float)set.kw[k];  // same expression as the untiled kernel: identical rounding
+        float* out = set.out[k];
 #pragma unroll
-    for (int oo = 0; oo < 4; ++oo) {
-        const int t = t0 + 4 * tid + oo;
-        if (t < nt) out[row * nt + t] = fmaxf(acc[oo], 0.f) / den;
+        for (int oo = 0; oo < 4; ++oo) {
+            const int t = t0 + 4 * tid + oo;
+            if (t < nt) out[row * nt + t] = fmaxf(acc[oo], 0.f) / den;
+        }
+        sk += set.nf[k] * kwp;
     }
 }
 

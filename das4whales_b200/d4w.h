@@ -193,6 +193,14 @@ int d4w_row_median(const float* dev_x, int nrows, size_t n, float* dev_median, v
 int d4w_row_max(const float* dev_x, int nrows, size_t n, float* dev_max, void* stream);
 int d4w_speccorr(const float* dev_S, int nx, int nf, int nt, const float* dev_K, int kw, const float* dev_median,
                  float* dev_out, void* stream);
+/* Median of each row of a band: row r is the n values at dev_x + r * ld (ld >= n); d4w_row_median is ld = n. */
+int d4w_row_median_ld(const float* dev_x, int nrows, size_t n, size_t ld, float* dev_median, void* stream);
+/* Several kernels against one band spectrogram dev_S [nx][nf][nt] (the union of their bands), S read once: for each
+ * k < nk (nk <= 8), d4w_speccorr of the slice S[:, f0[k] : f0[k] + nfk[k], :] with dev_K[k] [nfk[k]][kw[k]] and
+ * dev_median[k] [nx] into dev_out[k] [nx][nt], bit-equal to it.  The arrays are host arrays (of device pointers). */
+int d4w_speccorr_multi(const float* dev_S, int nx, int nf, int nt, int nk, const int* f0, const int* nfk,
+                       const float* const* dev_K, const int* kw, const float* const* dev_median, float* const* dev_out,
+                       void* stream);
 
 /* ---- peak picking -- detect.pick_times_env (detect.py:169-195, the find_peaks call :192) and detect.pick_times
  *      (:249-274, :271): scipy.signal.find_peaks(row, prominence=threshold) on every row of a [nx][ns] float32 matrix

@@ -268,31 +268,77 @@ def xcorr(t, f, Sxx, tvec, fvec, BlueKernel):
     return [t_scale, corr if tens else corr.to(torch.float64).cpu().numpy()]
 
 
+def spectrocorr_layout(fs, flims, kernels, win_size, overlap_pct, ns):
+    """Host side of the spectrogram-correlation detector for several kernels sharing one STFT, pure NumPy.
+    kernels: dicts {f0, f1, dur, bdwidth} (scripts/main_spectrodetect.py:103-104).  Each kernel widens flims as
+    detect.py:693-696 does (fmax -> f1 + 3 bdwidth when fmax - f1 < 2 bdwidth, fmin -> f0 - 3 bdwidth when
+    f0 - fmin < 2 bdwidth) and gets its buildkernel matrix on its own bins and the ns-sample record's frame times.
+    Returns (nperseg, nhop, bands, (b0, b1), per_kernel): bands[k] = the widened (fmin, fmax); b0 .. b1 the union of the
+    kernels' STFT bins (inclusive); per_kernel[k] = (offset of the kernel's first bin from b0, kernel [nf_k, kw_k], kw_k)."""
+    nperseg = int(win_size * fs)
+    nhop = int(np.floor(nperseg * (1 - overlap_pct)))
+    if nperseg < 1 or nhop < 1:
+        raise ValueError(f"window of {nperseg} samples with a hop of {nhop}: both must be >= 1")
+    nt = 1 + int(ns) // nhop
+    tt = np.linspace(0, int(ns) / fs, num=nt)
+    bands, bins, kers = [], [], []
+    for kernel in kernels:
+        fmin, fmax = flims
+        f1, f0, duration, bandwidth = kernel["f1"], kernel["f0"], kernel["dur"], kernel["bdwidth"]
+        if fmax - f1 < 2 * bandwidth:
+            fmax = f1 + 3 * bandwidth
+        if f0 - fmin < 2 * bandwidth:
+            fmin = f0 - 3 * bandwidth
+        ff, b0, b1 = _band_bins(nperseg, fs, fmin, fmax)
+        _, _, ker = buildkernel(f0, f1, bandwidth, duration, ff[b0:b1 + 1], tt, fs, fmin, fmax, plotflag=False)
+        if ker.shape[1] == 0:
+            raise ValueError(f"a kernel of {duration} s has no frames in a {int(ns) / fs:g} s record: buildkernel takes "
+                             f"its width from the frames with {7 * duration:g} s < t < {8 * duration:g} s")
+        bands.append((fmin, fmax))
+        bins.append((b0, b1))
+        kers.append(ker)
+    if not kers:
+        raise ValueError("spectrogram correlation needs at least one kernel")
+    u0, u1 = min(b[0] for b in bins), max(b[1] for b in bins)
+    return nperseg, nhop, bands, (u0, u1), [(b[0] - u0, k, k.shape[1]) for b, k in zip(bins, kers)]
+
+
+def _spectrocorr_device(xd, nperseg, nhop, union, per_kernel):
+    """The multi-kernel pass of spectrocorr_layout's layout on a float32 CUDA tensor [nx, ns], in channel chunks: one STFT
+    of the union band, one median per kernel over its slice of the band, one d4w_speccorr_multi.  -> list of [nx, nt]."""
+    import torch
+    nx, ns = xd.shape
+    b0, b1 = union
+    nf, nt = b1 - b0 + 1, 1 + ns // nhop
+    outs = [torch.empty((nx, nt), dtype=torch.float32, device=xd.device) for _ in per_kernel]
+    chunk = max(1, min(nx, _rows._MAX_ROWS, (2 << 30) // max(1, nf * nt * 4)))
+    for r0 in range(0, nx, chunk):
+        S = _rows.stft_mag(xd[r0:r0 + chunk], nperseg, nhop, b0, b1)
+        n = S.shape[0]
+        meds = [_rows.row_median_ld(S, n, ker.shape[0] * nt, nf * nt, off * nt) for off, ker, _ in per_kernel]
+        _rows.spectro_correlate_multi(S, [k for _, k, _ in per_kernel], [off for off, _, _ in per_kernel], meds,
+                                      outs=[o[r0:r0 + n] for o in outs])
+        del S
+    return outs
+
+
+def compute_cross_correlograms_spectrocorr(data, fs, flims, kernels, win_size, overlap_pct):
+    """compute_cross_correlogram_spectrocorr for several kernels (the HF and LF notes of scripts/main_spectrodetect.py:103-107)
+    from ONE STFT per channel: the STFT covers the union of the kernels' (widened) bands, each kernel is correlated with its
+    slice of it and normalised by the median of that slice, as its own call would do.  Returns a list with one correlogram
+    per kernel dict.  ndarray in -> float64 ndarrays out; CUDA tensor in -> float32 CUDA tensors out."""
+    xd = _to_device(data)
+    nperseg, nhop, _, union, per_kernel = spectrocorr_layout(fs, flims, kernels, win_size, overlap_pct, xd.shape[1])
+    outs = _spectrocorr_device(xd, nperseg, nhop, union, per_kernel)
+    return outs if _is_tensor(data) else [_to_host64(o) for o in outs]
+
+
 def compute_cross_correlogram_spectrocorr(data, fs, flims, kernel, win_size, overlap_pct):
     """Spectrogram-correlation detector over all channels (reference: detect.py:650-708): batched
     STFT of the band of interest, kernel correlation + frequency sum, median normalisation, all
-    on the GPU in channel chunks."""
-    import torch
+    on the GPU in channel chunks (the one-kernel case of compute_cross_correlograms_spectrocorr)."""
     nperseg = int(win_size * fs)
     nhop = int(np.floor(nperseg * (1 - overlap_pct)))
     noverlap = nperseg - nhop
     print(f'nperseg: {nperseg}, noverlap: {noverlap}, hop_length: {nhop}')
-    fmin, fmax = flims
-    f1, f0, duration, bandwidth = kernel["f1"], kernel["f0"], kernel["dur"], kernel["bdwidth"]
-    if fmax - f1 < 2 * bandwidth:
-        fmax = f1 + 3 * bandwidth
-    if f0 - fmin < 2 * bandwidth:
-        fmin = f0 - 3 * bandwidth
-    xd = _to_device(data)
-    nx, ns = xd.shape
-    ff, b0, b1 = _band_bins(nperseg, fs, fmin, fmax)
-    nt = 1 + ns // nhop
-    tt = np.linspace(0, ns / fs, num=nt)
-    _, _, ker = buildkernel(f0, f1, bandwidth, duration, ff[b0:b1 + 1], tt, fs, fmin, fmax, plotflag=False)
-    out = torch.empty((nx, nt), dtype=torch.float32, device=xd.device)
-    nf = b1 - b0 + 1
-    chunk = max(1, min(nx, (2 << 30) // max(1, nf * nt * 4)))
-    for r0 in range(0, nx, chunk):
-        S = _rows.stft_mag(xd[r0:r0 + chunk], nperseg, nhop, b0, b1)
-        out[r0:r0 + chunk] = _rows.spectro_correlate(S, ker)
-    return out if _is_tensor(data) else _to_host64(out)
+    return compute_cross_correlograms_spectrocorr(data, fs, flims, [kernel], win_size, overlap_pct)[0]

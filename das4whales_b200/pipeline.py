@@ -16,6 +16,10 @@ then the image-domain Gabor mask (improcess.gabor_detect, :78-169) and the scrip
 ("same") correlation of each masked channel divided by its maximum with the un-padded HF / LF notes, channels whose
 maximum is <= 0 skipped (detect.compute_cross_correlograms_same, :223-246) -- before the same threshold and picking (:252-266).
 
+`SpectroDetectPipeline` is scripts/main_spectrodetect.py:39-123: the same front end, then the HF and LF
+spectrogram-correlation correlograms from one sliding STFT (detect.compute_cross_correlograms_spectrocorr, :103-107) and
+find_peaks with an absolute prominence on the raw correlograms (detect.pick_times, :117-118); picks are in STFT frames.
+
 Only the raw counts go up (pinned int32, 4 bytes per sample) and only the picks come down; every intermediate matrix
 stays in HBM.  `stream(files)` overlaps the H2D copy of file i+1 with the processing of file i.
 """
@@ -30,8 +34,8 @@ from . import rows as _rows
 
 class _FilePipeline:
     """Shared part of the file pipelines: strain -> band-pass -> hybrid_ninf f-k filter on the device, the
-    threshold-and-pick tail, and the double-buffered upload of `stream`.  Subclasses set self.templates and implement
-    _correlograms(y) -> (list of [nx, ns] correlograms, extra results)."""
+    threshold-and-pick tail, and the double-buffered upload of `stream`.  Subclasses implement process_device(raw) on top
+    of _filtered and _pick (or their own picking tail)."""
 
     def __init__(self, nx, ns, selected_channels, dx, fs, scale_factor, device, fmin, fmax, mask_speeds, thres_frac,
                  prune_eps, bandpass):
@@ -41,7 +45,7 @@ class _FilePipeline:
         self.nx, self.ns, self.fs = int(nx), int(ns), float(fs)
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.scale_factor = float(scale_factor)
-        self.thres_frac = float(thres_frac)
+        self.thres_frac = None if thres_frac is None else float(thres_frac)      # None: the subclass picks by its own rule
         self.bandpass = bool(bandpass)
         with torch.cuda.device(self.device):
             self.mask = _dsp.hybrid_ninf_filter_design((nx, ns), selected_channels, dx, fs, *mask_speeds, fmin=fmin, fmax=fmax)
@@ -57,10 +61,13 @@ class _FilePipeline:
             x = _rows.sosfiltfilt(self.sos, x, padlen=3 * 17)
         return self.fk(x, out=x)
 
+    def _maxv(self, corr):
+        """max over all correlograms (0-dim device tensor; row_max clamps at 0)"""
+        rmax = self.torch.stack([_rows.row_max(c) for c in corr])                # [2, nx]
+        return _rows.row_max(rmax.reshape(1, -1))[0]
+
     def _pick(self, corr, with_snr):
-        torch = self.torch
-        rmax = torch.stack([_rows.row_max(c) for c in corr])                     # [2, nx]
-        maxv = _rows.row_max(rmax.reshape(1, -1))[0]
+        maxv = self._maxv(corr)
         thres = self.thres_frac * float(maxv.item())                             # main_mfdetect.py:95 (one scalar D2H)
         out = {"maxv": maxv, "threshold": thres}
         for name, c, thr in (("hf", corr[0], thres * 0.9), ("lf", corr[1], thres)):
@@ -185,6 +192,49 @@ class GaborDetectPipeline(_FilePipeline):
             return out
 
 
+KERNEL_HF = {"f0": 27., "f1": 17., "dur": 0.8, "bdwidth": 4.}          # scripts/main_spectrodetect.py:103
+KERNEL_LF = {"f0": 20., "f1": 14., "dur": 1.2, "bdwidth": 4.}          # :104
+
+
+class SpectroDetectPipeline(_FilePipeline):
+    """scripts/main_spectrodetect.py:39-123 on the device; the script's values are the defaults (flims = the band-pass band
+    fmin .. fmax, :102).  Same interface as MfDetectPipeline (process_device / process_file / stream).  Picks are STFT frame
+    indices; `spectro_fs` (frames per second, :123) converts them to seconds, `nt` is the number of frames per channel."""
+
+    def __init__(self, nx, ns, selected_channels, dx, fs, scale_factor, device=None, fmin=14., fmax=30.,
+                 mask_speeds=(1350., 1450., 3300, 3450), kernel_hf=None, kernel_lf=None, win_size=0.8, overlap_pct=0.95,
+                 threshold=14., prune_eps=0.0, bandpass=True):
+        super().__init__(nx, ns, selected_channels, dx, fs, scale_factor, device, fmin, fmax, mask_speeds, None,
+                         prune_eps, bandpass)
+        self.kernels = [dict(KERNEL_HF if kernel_hf is None else kernel_hf), dict(KERNEL_LF if kernel_lf is None else kernel_lf)]
+        self.flims = (float(fmin), float(fmax))
+        self.win_size, self.overlap_pct = float(win_size), float(overlap_pct)
+        self.threshold = float(threshold)
+        self.nperseg, self.nhop, self.bands, self.union, self.per_kernel = _detect.spectrocorr_layout(
+            self.fs, self.flims, self.kernels, self.win_size, self.overlap_pct, self.ns)
+        self.nt = 1 + self.ns // self.nhop
+        self.spectro_fs = self.nt / ((self.ns - 1) / self.fs)                # nt / time[-1], time = arange(ns) / fs
+
+    def process_device(self, raw, with_snr=False, with_intermediates=False):
+        """raw: int32 (or float32) CUDA tensor [nx, ns] of interrogator counts.  Returns a dict of DEVICE results:
+        picks_hf / picks_lf = (offsets int32 [nx + 1], idx int32 [n]) in frames, maxv (0-dim tensor), threshold, optionally
+        snr_hf / snr_lf (snr_tr_array(env=True) of each correlogram, :113-114) and, with_intermediates, the HF / LF
+        correlograms ("corr", [nx, nt] each)."""
+        torch = self.torch
+        with torch.cuda.device(self.device):
+            y = self._filtered(raw)
+            corr = _detect._spectrocorr_device(y, self.nperseg, self.nhop, self.union, self.per_kernel)
+            del y
+            out = {"maxv": self._maxv(corr), "threshold": self.threshold}             # :108
+            for name, c in zip(("hf", "lf"), corr):
+                out["picks_" + name] = _rows.find_peaks_device(c, self.threshold)    # pick_times, :117-118
+                if with_snr:
+                    out["snr_" + name] = _rows.snr(c, env=True)
+            if with_intermediates:
+                out["corr"] = corr
+            return out
+
+
 def process_file(raw, metadata, selected_channels, **kw):
     """Convenience wrapper: raw [nx, ns] counts + the reference's metadata dict (data_handle.get_acquisition_parameters:
     fs, dx, scale_factor) -> picks of the HF and LF fin-whale notes."""
@@ -198,4 +248,12 @@ def process_file_gabor(raw, metadata, selected_channels, **kw):
     scale_factor) -> picks of the HF and LF fin-whale notes of scripts/main_gabordetect.py."""
     nx, ns = raw.shape
     pipe = GaborDetectPipeline(nx, ns, selected_channels, metadata["dx"], metadata["fs"], metadata["scale_factor"], **kw)
+    return pipe.process_file(raw)
+
+
+def process_file_spectro(raw, metadata, selected_channels, **kw):
+    """Convenience wrapper of SpectroDetectPipeline: raw [nx, ns] counts + the reference's metadata dict (fs, dx,
+    scale_factor) -> frame-index picks of the HF and LF notes of scripts/main_spectrodetect.py."""
+    nx, ns = raw.shape
+    pipe = SpectroDetectPipeline(nx, ns, selected_channels, metadata["dx"], metadata["fs"], metadata["scale_factor"], **kw)
     return pipe.process_file(raw)

@@ -377,6 +377,64 @@ def row_median(x2d):
     return out
 
 
+def row_median_ld(x, nrows, n, ld, offset=0):
+    """np.median of x.flat[offset + r * ld : offset + r * ld + n] for r < nrows, x a contiguous non-negative float32 CUDA
+    tensor.  For the band of rows f0 .. f0 + m - 1 of every channel of a spectrogram [nx, nf, nt]: nrows = nx, n = m * nt,
+    ld = nf * nt, offset = f0 * nt.  Returns [nrows] float32."""
+    torch = _torch()
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()):
+        raise ValueError("expected a contiguous float32 CUDA tensor")
+    nrows, n, ld, offset = int(nrows), int(n), int(ld), int(offset)
+    if nrows < 1 or n < 1 or ld < n or offset < 0 or offset + (nrows - 1) * ld + n > x.numel():
+        raise ValueError(f"row_median_ld: {nrows} rows of {n} values at stride {ld} from {offset} do not fit {x.numel()} values")
+    out = torch.empty(nrows, dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device.index):
+        _lib.check(_lib.lib().d4w_row_median_ld(_lib.ffi.cast("float*", x.data_ptr() + 4 * offset), nrows, n, ld,
+                                                _lib.ptr(out, "float*"), _lib.stream_ptr()), "row_median_ld")
+    return out
+
+
+SPECCORR_MAX_KERNELS = 8        # kernels per d4w_speccorr_multi call (csrc/rows_kernels.cuh, kScMaxKernels)
+
+
+def spectro_correlate_multi(S, kernels, offsets, medians, outs=None):
+    """spectro_correlate of several kernels against one band spectrogram S [nx, nf, nt] (float32 CUDA), S read once per
+    group of up to 8 kernels: kernel k ([nf_k, kw_k]) covers the rows offsets[k] .. offsets[k] + nf_k - 1 of S and is
+    normalised by medians[k] ([nx] float32 CUDA).  Output k is bit-equal to spectro_correlate(S[:, o:o + nf_k], kernel,
+    median).  outs: optional contiguous [nx, nt] float32 tensors to write.  Any number of rows.  Returns the list of outputs."""
+    torch = _torch()
+    if not (isinstance(S, torch.Tensor) and S.is_cuda and S.dtype == torch.float32 and S.is_contiguous() and S.ndim == 3):
+        raise ValueError("expected a contiguous float32 CUDA tensor [channels, bins, frames]")
+    nx, nf, nt = S.shape
+    Ks = [torch.from_numpy(np.ascontiguousarray(k, dtype=np.float32)).to(S.device) for k in kernels]
+    if len(Ks) == 0 or len(Ks) != len(offsets) or len(Ks) != len(medians):
+        raise ValueError("spectro_correlate_multi: one offset and one median per kernel")
+    for K, o in zip(Ks, offsets):
+        if K.ndim != 2 or K.shape[1] < 1 or o < 0 or o + K.shape[0] > nf:
+            raise ValueError(f"kernel of shape {tuple(K.shape)} at bin offset {o} does not fit a band of {nf} bins")
+    if any(m.dtype != torch.float32 or not m.is_cuda or tuple(m.shape) != (nx,) for m in medians):
+        raise ValueError(f"medians must be float32 CUDA tensors of {nx} values")
+    if outs is None:
+        outs = [torch.empty((nx, nt), dtype=torch.float32, device=S.device) for _ in Ks]
+    if len(outs) != len(Ks) or any(o.dtype != torch.float32 or tuple(o.shape) != (nx, nt) or not o.is_contiguous() for o in outs):
+        raise ValueError(f"outs must be contiguous float32 CUDA tensors [{nx}, {nt}]")
+    ffi, L = _lib.ffi, _lib.lib()
+    with torch.cuda.device(S.device.index):
+        for g0 in range(0, len(Ks), SPECCORR_MAX_KERNELS):
+            g = range(g0, min(len(Ks), g0 + SPECCORR_MAX_KERNELS))
+            f0 = ffi.new("int[]", [int(offsets[k]) for k in g])
+            nfk = ffi.new("int[]", [Ks[k].shape[0] for k in g])
+            kw = ffi.new("int[]", [Ks[k].shape[1] for k in g])
+            kp = ffi.new("float*[]", [_lib.ptr(Ks[k], "float*") for k in g])
+            for r0 in range(0, nx, _MAX_ROWS):
+                r1 = min(nx, r0 + _MAX_ROWS)
+                mp = ffi.new("float*[]", [_lib.ptr(medians[k][r0:r1], "float*") for k in g])
+                op = ffi.new("float*[]", [_lib.ptr(outs[k][r0:r1], "float*") for k in g])
+                _lib.check(L.d4w_speccorr_multi(_lib.ptr(S[r0:r1], "float*"), r1 - r0, nf, nt, len(g), f0, nfk, kp, kw, mp, op,
+                                                _lib.stream_ptr()), "speccorr_multi")
+    return outs
+
+
 def spectro_correlate(S, kernel, median=None):
     """detect.xcorr2d for a batch: S [nx, nf, nt] float32 CUDA (un-normalised magnitudes are fine:
     the max-normalisation of get_sliced_nspectrogram cancels against the median), kernel [nf, kw]."""
