@@ -10,7 +10,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libd4w.so")
-SOURCES = ["d4w_fk.cu", "d4w_rows.cu", "d4w_xcorr_same.cu", "d4w_image.cu"]
+SOURCES = ["d4w_fk.cu", "d4w_rows.cu", "d4w_xcorr_same.cu", "d4w_image.cu", "d4w_noise.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-std=c++17", "-O3", "--expt-relaxed-constexpr"] + GENCODE + [
               "-lineinfo", "-Xcompiler", "-fPIC", "-Wno-deprecated-gpu-targets"]

@@ -4,6 +4,7 @@
 #include <cstring>
 #include "d4w_common.hpp"
 #include "fk_hostplan.hpp"
+#include "row_plan.hpp"
 #include "rows_kernels.cuh"
 #include "xcorr_launch.cuh"
 
@@ -124,18 +125,7 @@ extern "C" int d4w_xcorr(d4w_fft_plan* p, const float* x, int nx, int ns, int va
 }
 
 // ------------------------------------------------------------------ Hilbert envelope / envelope SNR
-struct d4w_row_plan {
-    int ns = 0, device = 0, t1 = 1, t2 = 0;
-    RowParams row{};
-    float2 *d_tw = nullptr, *d_twT = nullptr;
-    float* d_hilbert = nullptr;
-    float* d_sgn = nullptr;      // sgn(f)/ns in k_row_mid_fused's table order (two-rows-per-transform route)
-    size_t row_smem = 0;
-    int fused = 0;               // split rows: middle pass by k_row_mid_fused (weights stored in its table order)
-    // chirp-z rows (no mixed-radix split of ns): t1 x t2 = czt_m is the convolution length, hilbert_czt.cuh
-    int czt_m = 0, pair = 0;
-    float2 *d_chirp = nullptr, *d_bhat = nullptr, *d_bhatc = nullptr;
-};
+// struct d4w_row_plan: row_plan.hpp
 
 // plan for a row length the time-axis planner rejects: chirp-z transform over an m-point convolution
 static int row_plan_create_czt(d4w_row_plan** out, int ns, int device, const cudaDeviceProp& prop) {

@@ -326,6 +326,52 @@ def snr_tr_array(trace, env=False):
     return y if _is_tensor(trace) else _to_host64(y)
 
 
+# ------------------------------------------------------------------------------ cable noise profile
+NOISE_PROFILE_KEYS = ("med", "mean", "std", "std_med_diff", "SNR_1d", "noise_power", "noise_power_db", "noise_mean")
+
+
+def noise_window(ns, fs, tnoise=(19., 26.)):
+    """Sample range [i0, i1) of the noise window, int(t * fs) for each end (scripts/main_bathynoise.py:251).
+    Raises ValueError for an empty window or one outside [0, ns]."""
+    i0, i1 = (int(t * fs) for t in tnoise)
+    if not 0 <= i0 < i1 <= int(ns):
+        raise ValueError(f"noise window {tuple(tnoise)} s -> samples [{i0}, {i1}) is empty or outside [0, {int(ns)}]")
+    return i0, i1
+
+
+def noise_profile_from_stats(full, win, p_ref=1e-11):
+    """The profile of scripts/main_bathynoise.py:183-194, :257-259 from two rows.env_stats records ([nx, 5] float64,
+    ndarrays or tensors): `full` of the whole rows, `win` of the noise window.  Division and log follow IEEE, as NumPy: a
+    zero channel gives SNR_1d = nan and noise_power_db = -inf."""
+    if _is_tensor(full):
+        import torch
+        sqrt, log10, col = torch.sqrt, torch.log10, (lambda a, j: a[:, j].contiguous())
+    else:
+        sqrt, log10, col = np.sqrt, np.log10, (lambda a, j: np.ascontiguousarray(a[:, j], dtype=np.float64))
+    med, std = col(full, 0), sqrt(col(full, 4))
+    noise_power = col(win, 3)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return {"med": med, "mean": col(full, 1), "std": std, "std_med_diff": std - med, "SNR_1d": 20 * log10(std / med),
+                "noise_power": noise_power, "noise_power_db": 10 * log10(noise_power / p_ref ** 2),
+                "noise_mean": col(win, 1)}
+
+
+def cable_noise_profile(trace, fs, tnoise=(19., 26.), p_ref=1e-11):
+    """Per-channel noise floor of scripts/main_bathynoise.py:183-194, :248-259 for the f-k filtered strain `trace`
+    [nx, ns]: median and mean of the Hilbert envelope (med, mean), the population std, std_med_diff = std - med,
+    SNR_1d = 20 log10(std / med), and over the window tnoise (seconds, int(t * fs) samples) noise_power = mean(x^2),
+    noise_power_db = 10 log10(noise_power / p_ref^2) and noise_mean = the mean envelope of the window alone.
+    Returns a dict of NOISE_PROFILE_KEYS: float64 ndarrays for an ndarray in, float64 CUDA tensors for a tensor in.
+    Only [nx]-long vectors leave the GPU."""
+    i0, i1 = noise_window(np.shape(trace)[-1], fs, tnoise)
+    xd = _to_device(trace)
+    full = _rows.env_stats(xd)
+    win = _rows.env_stats(xd, i0, i1 - i0)
+    if _is_tensor(trace):
+        return noise_profile_from_stats(full, win, p_ref)
+    return noise_profile_from_stats(full.cpu().numpy(), win.cpu().numpy(), p_ref)
+
+
 # Channel counts with a prime factor > 61 go through the chirp-z column transform of length M = the smallest 2^a 3^b 5^c
 # >= 2 nx - 1, and one M-point complex column must fit the 200 KB column budget: M <= 25 600, so nx <= 12 800
 # (csrc/fk_hostplan.hpp, czt_max_channels).

@@ -20,6 +20,10 @@ maximum is <= 0 skipped (detect.compute_cross_correlograms_same, :223-246) -- be
 spectrogram-correlation correlograms from one sliding STFT (detect.compute_cross_correlograms_spectrocorr, :103-107) and
 find_peaks with an absolute prominence on the raw correlograms (detect.pick_times, :117-118); picks are in STFT frames.
 
+`NoiseProfilePipeline` is scripts/main_bathynoise.py:122-259: the same front end, then the per-channel noise profile
+(envelope median and mean, std, SNR_1d, and the power and mean envelope of a noise window) from two envelope-statistics
+passes (rows.env_stats); it yields [nx]-long float64 vectors instead of picks.
+
 Only the raw counts go up (pinned int32, 4 bytes per sample) and only the picks come down; every intermediate matrix
 stays in HBM.  `stream(files)` overlaps the H2D copy of file i+1 with the processing of file i.
 """
@@ -78,6 +82,11 @@ class _FilePipeline:
                 out["snr_" + name] = _rows.snr(c, env=True)
         return out
 
+    def _to_host(self, res):
+        """process_device's result -> what process_file / stream yield: host pick arrays, maxv and threshold"""
+        return {"picks_hf": self.picks_to_host(res["picks_hf"]), "picks_lf": self.picks_to_host(res["picks_lf"]),
+                "maxv": float(res["maxv"].item()), "threshold": res["threshold"]}
+
     @staticmethod
     def picks_to_host(picks):
         """(offsets, idx) on the device -> array([[channel ...], [sample ...]]) like detect.convert_pick_times."""
@@ -99,8 +108,9 @@ class _FilePipeline:
         return next(self.stream([raw_host]))
 
     def stream(self, files):
-        """Iterate over host arrays / tensors; yields {"picks_hf", "picks_lf", "maxv", "threshold"} per file with the H2D
-        copy of the next file running on a second stream under the processing of the current one."""
+        """Iterate over host arrays / tensors; yields the host results of each file (_to_host: {"picks_hf", "picks_lf",
+        "maxv", "threshold"} for the detectors) with the H2D copy of the next file running on a second stream under the
+        processing of the current one."""
         torch = self.torch
         if self._h2d is None:
             self._h2d = torch.cuda.Stream(device=self.device)
@@ -131,9 +141,7 @@ class _FilePipeline:
             # previous user of that staging buffer -- and then runs under this file's processing
             pending = upload((i + 1) % 2, nxt) if nxt is not None else None
             cur_stream.wait_event(ev)
-            res = self.process_device(dst)
-            yield {"picks_hf": self.picks_to_host(res["picks_hf"]), "picks_lf": self.picks_to_host(res["picks_lf"]),
-                   "maxv": float(res["maxv"].item()), "threshold": res["threshold"]}
+            yield self._to_host(self.process_device(dst))
             i += 1
 
 
@@ -235,6 +243,37 @@ class SpectroDetectPipeline(_FilePipeline):
             return out
 
 
+class NoiseProfilePipeline(_FilePipeline):
+    """scripts/main_bathynoise.py:122-259 on the device; the script's values are the defaults.  The same front end as the
+    detectors, then the per-channel noise profile of dsp.cable_noise_profile: two rows.env_stats passes (the whole rows and
+    the noise window tnoise, int(t * fs) samples), so only [nx]-long vectors leave the GPU.  process_file / stream yield
+    dicts of float64 ndarrays keyed by dsp.NOISE_PROFILE_KEYS."""
+
+    def __init__(self, nx, ns, selected_channels, dx, fs, scale_factor, device=None, fmin=14., fmax=30.,
+                 mask_speeds=(1350., 1450., 3300, 3450), tnoise=(19., 26.), p_ref=1e-11, prune_eps=0.0, bandpass=True):
+        self.i0, self.i1 = _dsp.noise_window(ns, fs, tnoise)
+        self.p_ref = float(p_ref)
+        super().__init__(nx, ns, selected_channels, dx, fs, scale_factor, device, fmin, fmax, mask_speeds, None,
+                         prune_eps, bandpass)
+
+    def process_device(self, raw, with_image=False):
+        """raw: int32 (or float32) CUDA tensor [nx, ns] of interrogator counts.  Returns a dict of float64 CUDA tensors [nx]
+        keyed by dsp.NOISE_PROFILE_KEYS and, with_image, "image" = |hilbert(trf_fk)| / std(trf_fk) (float32 [nx, ns], the
+        t-x plot of :139)."""
+        torch = self.torch
+        with torch.cuda.device(self.device):
+            y = self._filtered(raw)
+            full = _rows.env_stats(y)
+            win = _rows.env_stats(y, self.i0, self.i1 - self.i0)
+            out = _dsp.noise_profile_from_stats(full, win, self.p_ref)
+            if with_image:
+                out["image"] = _rows.envelope_over_std(y)
+            return out
+
+    def _to_host(self, res):
+        return {k: v.cpu().numpy() for k, v in res.items()}
+
+
 def process_file(raw, metadata, selected_channels, **kw):
     """Convenience wrapper: raw [nx, ns] counts + the reference's metadata dict (data_handle.get_acquisition_parameters:
     fs, dx, scale_factor) -> picks of the HF and LF fin-whale notes."""
@@ -256,4 +295,12 @@ def process_file_spectro(raw, metadata, selected_channels, **kw):
     scale_factor) -> frame-index picks of the HF and LF notes of scripts/main_spectrodetect.py."""
     nx, ns = raw.shape
     pipe = SpectroDetectPipeline(nx, ns, selected_channels, metadata["dx"], metadata["fs"], metadata["scale_factor"], **kw)
+    return pipe.process_file(raw)
+
+
+def process_file_noise(raw, metadata, selected_channels, **kw):
+    """Convenience wrapper of NoiseProfilePipeline: raw [nx, ns] counts + the reference's metadata dict (fs, dx,
+    scale_factor) -> the per-channel noise profile of scripts/main_bathynoise.py (float64 ndarrays)."""
+    nx, ns = raw.shape
+    pipe = NoiseProfilePipeline(nx, ns, selected_channels, metadata["dx"], metadata["fs"], metadata["scale_factor"], **kw)
     return pipe.process_file(raw)

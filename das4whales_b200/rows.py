@@ -260,6 +260,37 @@ def envelope_over_std(x):
     return _hilbert(x, 3, stats)
 
 
+ENV_STATS_FIELDS = ("median_env", "mean_env", "mean", "mean_sq", "var")
+
+
+def env_stats(x, t0=0, n=None):
+    """Envelope and moment statistics of the window x[:, t0:t0 + n] of every row (scripts/main_bathynoise.py:183-189,
+    :257-259), read in place.  x: contiguous float32 CUDA tensor [nx, ns]; n defaults to ns - t0.  Returns a float64 CUDA
+    tensor [nx, 5] with the columns ENV_STATS_FIELDS: median and mean of |scipy.signal.hilbert(window)|, and the mean, mean
+    square and population variance of the window.  The Hilbert transform is that of the window alone."""
+    torch = _torch()
+    dev = _check_input(x)
+    nx, ns = x.shape
+    t0 = int(t0)
+    n = ns - t0 if n is None else int(n)
+    if t0 < 0 or n < 1 or t0 + n > ns:
+        raise ValueError(f"env_stats: window [{t0}, {t0 + n}) is empty or outside the {ns} samples of a row")
+    plan = row_plan(n, dev)
+    out = torch.empty((nx, 5), dtype=torch.float64, device=x.device)
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        # the workspace holds the envelope and the Hilbert workspace of a chunk of rows: chunk so that it stays bounded, as _hilbert
+        per_row = max(1, int(L.d4w_env_stats_workspace_bytes(plan.ptr, 1, ns)))
+        max_rows = max(1, min(nx, (8 << 30) // per_row))
+        ws = torch.empty(int(L.d4w_env_stats_workspace_bytes(plan.ptr, max_rows, ns)), dtype=torch.uint8, device=x.device)
+        base = x.data_ptr() + 4 * t0
+        for r0 in range(0, nx, max_rows):
+            r1 = min(nx, r0 + max_rows)
+            _lib.check(L.d4w_env_stats(plan.ptr, _lib.ffi.cast("float*", base + 4 * r0 * ns), r1 - r0, ns,
+                                       _lib.ptr(out[r0:r1], "double*"), _lib.ptr(ws), _lib.stream_ptr()), "env_stats")
+    return out
+
+
 def row_fft_mag(x, nfft, scale):
     """|numpy.fft.fft(x, nfft)| * scale in fftshift order for every row (dsp.get_fx, dsp.py:35-37)."""
     torch = _torch()

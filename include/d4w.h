@@ -161,6 +161,14 @@ size_t d4w_row_workspace_bytes(const d4w_row_plan* plan, int nx);
 int d4w_row_plan_info(const d4w_row_plan* plan, int* t1, int* t2, int* czt_m);
 int d4w_hilbert(d4w_row_plan* plan, const float* dev_x, float* dev_out, int nx, void* dev_workspace, int mode,
                 const double* dev_stats, void* stream);
+/* Envelope and moment statistics of a row window (scripts/main_bathynoise.py:183-189, :257-259).  Row r is the n samples at
+ * dev_x + r * ld (ld >= n), n = the row plan's length (any n up to 128 000, as d4w_hilbert).  out: double[nrows][5] =
+ * {median |hilbert(x)|, mean |hilbert(x)|, mean x, mean x^2, population variance of x}; a row of variance 0 is constant and
+ * gets the envelope statistics |mean x| exactly (0 for a zero channel).
+ * dev_workspace: d4w_env_stats_workspace_bytes(plan, nrows, ld) bytes (the envelope of up to 65 535 rows, and a dense copy of
+ * the window when ld != n).  Any nrows >= 1. */
+size_t d4w_env_stats_workspace_bytes(const d4w_row_plan* plan, int nrows, size_t ld);
+int d4w_env_stats(d4w_row_plan* plan, const float* dev_x, int nrows, size_t ld, double* dev_out, void* dev_workspace, void* stream);
 
 /* ---- zero-phase IIR: dsp.bp_filt = scipy.signal.filtfilt (dsp.py:859-880) and the caller-side
  *      scipy.signal.sosfiltfilt(sos, trace, axis=1) (Example.py:55).  host_sos: double[nsec][6],
