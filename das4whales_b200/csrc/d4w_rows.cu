@@ -23,21 +23,18 @@ extern "C" int d4w_fft_plan_create(d4w_fft_plan** out, int n, int device) {
     auto p = new d4w_fft_plan();
     p->n = n; p->device = device; p->smem_cap = prop.sharedMemPerBlockOptin;
     std::string err;
-    // overlap-save block lengths (rows.py _pick_block): big even radix first, small odd radix last suits k_xcorr_fused
-    const char* forced = std::getenv("D4W_BLOCK_PLAN");
-    // dual-lane matched filter (default): radices <= 10 only (register budget of two 256-thread CTAs per SM)
-    const bool dual_blocks = env_int("D4W_XCORR_DUAL", 1) != 0;
-    const char* pref = dual_blocks ? (n == 1250 ? "10,5,5,5" : n == 2500 ? "10,10,5,5" : n == 5000 ? "10,10,10,5" : n == 10000 ? "10,10,10,10" : nullptr)
-                                   : (n == 1250 ? "10,25,5" : n == 2500 ? "20,25,5" : n == 5000 ? "20,10,25" : n == 10000 ? "20,20,25" : nullptr);
-    bool have = false;
-    if (forced && *forced) have = make_plan_from_string(n, forced, p->pl);
-    if (!have && pref && env_int("D4W_XCORR_FUSED", 1)) have = make_plan_from_string(n, pref, p->pl);
-    if (!have && !make_plan(n, env_int("D4W_BLOCK_MAX_RADIX", 25), p->pl, err, 128, 16)) { delete p; return fail(D4W_ERR_UNSUPPORTED, err); }
+    // overlap-save block lengths (rows.py _pick_block) for the dual-lane matched filter: radices <= 10 only (register budget
+    // of two 256-thread CTAs per SM), in-register first and last radix for k_xcorr_fused / k_xcorr_dual
+    const char* pref = n == 1250 ? "10,5,5,5" : n == 2500 ? "10,10,5,5" : n == 5000 ? "10,10,10,5" : n == 10000 ? "10,10,10,10" : nullptr;
+    if (!(pref && make_plan_from_string(n, pref, p->pl)) && !make_plan(n, 25, p->pl, err, 128, 16)) {
+        delete p;
+        return fail(D4W_ERR_UNSUPPORTED, err);
+    }
     p->pos2k = make_pos2freq(p->pl);
     p->tab2k = p->pos2k;
     {
         const int nst = p->pl.nstages;
-        if (env_int("D4W_XCORR_FUSED", 1) && nst >= 2 && row_radix_inreg(p->pl.radix[0]) && row_radix_inreg(p->pl.radix[nst - 1])) {
+        if (nst >= 2 && row_radix_inreg(p->pl.radix[0]) && row_radix_inreg(p->pl.radix[nst - 1])) {
             p->fused = 1;
             const int rl = p->pl.radix[nst - 1], G = n / rl;
             for (int m = 0; m < rl; ++m)
@@ -45,7 +42,7 @@ extern "C" int d4w_fft_plan_create(d4w_fft_plan** out, int n, int device) {
         }
     }
     std::vector<int> tpos;
-    if (n == kPfaN && env_int("D4W_XCORR_PFA", 1)) {
+    if (n == kPfaN) {
         // prime-factor plan: positions are [5][7][8][9] digits; table order of the fused last dimension (radix 9)
         p->pfa = 1; p->fused = 0;
         pfa_build_maps(tpos, p->pos2k);
@@ -136,7 +133,7 @@ static int row_plan_create_czt(d4w_row_plan** out, int ns, int device, const cud
     p->ns = ns; p->device = device; p->t1 = hp.t1; p->t2 = hp.t2; p->row_smem = hp.row_smem;
     p->row.pl = hp.rowpl; p->row.t1 = hp.t1; p->row.t2 = hp.t2;
     p->fused = cz.fused; p->czt_m = cz.m;
-    p->pair = (hp.t1 > 1 && env_int("D4W_HILBERT_PAIR", 1)) ? 1 : 0;
+    p->pair = hp.t1 > 1 ? 1 : 0;
     std::vector<float2> bc(cz.bhat.size());
     for (size_t i = 0; i < bc.size(); ++i) bc[i] = make_float2(cz.bhat[i].x, -cz.bhat[i].y);
     cudaError_t e = upload(&p->d_tw, hp.tw_row);
@@ -163,7 +160,7 @@ extern "C" int d4w_row_plan_create(d4w_row_plan** out, int ns, int device) {
     D4W_CUDA_TRY(cudaGetDeviceProperties(&prop, device));
     FkHostPlan hp; std::string err;
     // the envelope keeps k_row_mid_fused: 10 000 x 120 000 on an H100 took 15.5 ms with it and 16.9 ms with k_row_mid
-    // (two rows per transform both ways; one row per transform: 25.1 ms)
+    // (two rows per transform both ways; one row per transform, no longer built: 25.1 ms)
     // a length with no T1 x T2 split (a prime factor > 61, or T2 too long) goes through the chirp-z rows
     if (build_fk_hostplan(1, ns, prop.sharedMemPerBlockOptin, hp, err, /*allow_row_dual=*/false, /*row_fused_default=*/1))
         return row_plan_create_czt(out, ns, device, prop);
@@ -173,6 +170,7 @@ extern "C" int d4w_row_plan_create(d4w_row_plan** out, int ns, int device) {
     // analytic-signal weights of scipy.signal.hilbert (N = ns, no padding), scaled by 1/ns, transform order
     std::vector<float> h((size_t)ns);
     p->fused = (hp.t1 > 1 && hp.row_fused) ? 1 : 0;
+    p->pair = hp.t1 > 1 ? 1 : 0;
     const std::vector<int>& order = p->fused ? hp.pos2k_row_tab : hp.pos2k_row;
     for (int kt1 = 0; kt1 < hp.t1; ++kt1)
         for (int pos = 0; pos < hp.t2; ++pos) {
@@ -182,9 +180,9 @@ extern "C" int d4w_row_plan_create(d4w_row_plan** out, int ns, int device) {
             else wgt = (f == 0) ? 1.0 : (f <= (ns - 1) / 2 ? 2.0 : 0.0);
             h[(size_t)kt1 * hp.t2 + pos] = (float)(wgt / ns);
         }
-    // two real rows per complex transform; sg inherits h's table order, so either middle-pass kernel can apply it
+    // split rows: two real rows per complex transform; sg inherits h's table order, so either middle-pass kernel can apply it
     std::vector<float> sg;
-    if (hp.t1 > 1 && env_int("D4W_HILBERT_PAIR", 1)) {
+    if (p->pair) {
         sg.resize((size_t)ns);
         for (size_t i = 0; i < sg.size(); ++i) sg[i] = h[i] - (float)(1.0 / ns);      // h - 1: 0 at DC / Nyquist, +-1 elsewhere
     }
@@ -212,9 +210,8 @@ extern "C" int d4w_row_plan_destroy(d4w_row_plan* p) {
 
 extern "C" size_t d4w_row_workspace_bytes(const d4w_row_plan* p, int nx) {
     if (!p || p->t1 == 1) return 16;
-    const bool pair = p->czt_m ? p->pair != 0 : p->d_sgn != nullptr;
-    const size_t rows = pair ? (size_t)(nx + 1) / 2 : (size_t)nx;      // two real rows share one complex workspace row
-    return rows * (size_t)(p->czt_m ? p->czt_m : p->ns) * sizeof(float2);
+    // two real rows share one complex workspace row
+    return (size_t)(nx + 1) / 2 * (size_t)(p->czt_m ? p->czt_m : p->ns) * sizeof(float2);
 }
 
 extern "C" int d4w_row_plan_info(const d4w_row_plan* p, int* t1, int* t2, int* czt_m) {
@@ -238,38 +235,27 @@ static int hilbert_czt(d4w_row_plan* p, const float* x, float* out, int nx, void
     }
     if (!workspace) return fail(D4W_ERR_ARG, "d4w_hilbert: workspace required for split rows");
     float2* w = (float2*)workspace;
-    const int nrow = p->pair ? (nx + 1) / 2 : nx, thr = 128;
-    const dim3 g((p->t2 + thr - 1) / thr, nrow), gm(p->t1, nrow);
+    const int npair = (nx + 1) / 2, thr = 128;
+    const dim3 g((p->t2 + thr - 1) / thr, npair), gm(p->t1, npair);
     auto mid = [&](const float2* tab) {
         if (p->fused) k_row_mid_fused_c<<<gm, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->czt_m, tab, (size_t)0);
         else k_row_mid_c<<<gm, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->czt_m, tab, (size_t)0);
     };
-    switch (p->t1) {
-#define D4W_HC(T) case T: k_hczt_fwd<T><<<g, thr, 0, stream>>>(hz, x, w); break;
-        D4W_HC(2) D4W_HC(3) D4W_HC(4) D4W_HC(5) D4W_HC(6) D4W_HC(8) D4W_HC(10) D4W_HC(12) D4W_HC(15) D4W_HC(16) D4W_HC(20) D4W_HC(25)
-#undef D4W_HC
-        default: return fail(D4W_ERR_UNSUPPORTED, "row split radix not built");
-    }
-    D4W_CHECK_LAUNCH("k_hczt_fwd");
-    mid(p->d_bhat);
-    D4W_CHECK_LAUNCH("k_row_mid_c");
-    switch (p->t1) {
-#define D4W_HC(T) case T: k_hczt_turn<T><<<g, thr, 0, stream>>>(hz, w); break;
-        D4W_HC(2) D4W_HC(3) D4W_HC(4) D4W_HC(5) D4W_HC(6) D4W_HC(8) D4W_HC(10) D4W_HC(12) D4W_HC(15) D4W_HC(16) D4W_HC(20) D4W_HC(25)
-#undef D4W_HC
-        default: return fail(D4W_ERR_UNSUPPORTED, "row split radix not built");
-    }
-    D4W_CHECK_LAUNCH("k_hczt_turn");
-    mid(p->d_bhatc);
-    D4W_CHECK_LAUNCH("k_row_mid_c");
-    switch (p->t1) {
-#define D4W_HC(T) case T: k_hczt_inv<T><<<g, thr, 0, stream>>>(hz, w, x, out, mode, dev_stats); break;
-        D4W_HC(2) D4W_HC(3) D4W_HC(4) D4W_HC(5) D4W_HC(6) D4W_HC(8) D4W_HC(10) D4W_HC(12) D4W_HC(15) D4W_HC(16) D4W_HC(20) D4W_HC(25)
-#undef D4W_HC
-        default: return fail(D4W_ERR_UNSUPPORTED, "row split radix not built");
-    }
-    D4W_CHECK_LAUNCH("k_hczt_inv");
-    return D4W_OK;
+    const int rc = with_t1(p->t1, [&](auto tc) -> int {
+        constexpr int T1 = decltype(tc)::value;
+        k_hczt_fwd<T1><<<g, thr, 0, stream>>>(hz, x, w);
+        D4W_CHECK_LAUNCH("k_hczt_fwd");
+        mid(p->d_bhat);
+        D4W_CHECK_LAUNCH("k_row_mid_c");
+        k_hczt_turn<T1><<<g, thr, 0, stream>>>(hz, w);
+        D4W_CHECK_LAUNCH("k_hczt_turn");
+        mid(p->d_bhatc);
+        D4W_CHECK_LAUNCH("k_row_mid_c");
+        k_hczt_inv<T1><<<g, thr, 0, stream>>>(hz, w, x, out, mode, dev_stats);
+        D4W_CHECK_LAUNCH("k_hczt_inv");
+        return D4W_OK;
+    });
+    return rc == D4W_ERR_UNSUPPORTED ? fail(rc, "row split radix not built") : rc;
 }
 
 extern "C" int d4w_hilbert(d4w_row_plan* p, const float* x, float* out, int nx, void* workspace, int mode,
@@ -287,52 +273,22 @@ extern "C" int d4w_hilbert(d4w_row_plan* p, const float* x, float* out, int nx, 
         return D4W_OK;
     }
     if (!workspace) return fail(D4W_ERR_ARG, "d4w_hilbert: workspace required for split rows");
-    if (p->d_sgn) {                                              // two real rows per complex transform
-        float2* w2 = (float2*)workspace;
-        const int npair = (nx + 1) / 2, thr = 128;
-        dim3 g2((p->t2 + thr - 1) / thr, npair);
-        switch (p->t1) {
-#define D4W_HC(T) case T: k_hsplit_fwd2<T><<<g2, thr, 0, stream>>>(x, nx, p->ns, w2, p->t2, p->d_twT); break;
-            D4W_HC(2) D4W_HC(3) D4W_HC(4) D4W_HC(5) D4W_HC(6) D4W_HC(8) D4W_HC(10) D4W_HC(12) D4W_HC(15) D4W_HC(16) D4W_HC(20) D4W_HC(25)
-#undef D4W_HC
-            default: return fail(D4W_ERR_UNSUPPORTED, "row split radix not built");
-        }
+    // two real rows per complex transform
+    float2* w = (float2*)workspace;
+    const int npair = (nx + 1) / 2, thr = 128;
+    const dim3 g((p->t2 + thr - 1) / thr, npair), gm(p->t1, npair);
+    const int rc = with_t1(p->t1, [&](auto tc) -> int {
+        constexpr int T1 = decltype(tc)::value;
+        k_hsplit_fwd2<T1><<<g, thr, 0, stream>>>(x, nx, p->ns, w, p->t2, p->d_twT);
         D4W_CHECK_LAUNCH("k_hsplit_fwd2");
-        dim3 gm(p->t1, npair);
-        if (p->fused) k_row_mid_fused<<<gm, 256, p->row_smem, stream>>>(p->row, w2, (size_t)p->ns, p->d_sgn, (size_t)0);
-        else k_row_mid<<<gm, 256, p->row_smem, stream>>>(p->row, w2, (size_t)p->ns, p->d_sgn, (size_t)0);
+        if (p->fused) k_row_mid_fused<<<gm, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->ns, p->d_sgn, (size_t)0);
+        else k_row_mid<<<gm, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->ns, p->d_sgn, (size_t)0);
         D4W_CHECK_LAUNCH("k_row_mid");
-        switch (p->t1) {
-#define D4W_HC(T) case T: k_hsplit_inv2<T><<<g2, thr, 0, stream>>>(w2, x, nx, p->ns, out, p->t2, p->d_twT, mode, dev_stats); break;
-            D4W_HC(2) D4W_HC(3) D4W_HC(4) D4W_HC(5) D4W_HC(6) D4W_HC(8) D4W_HC(10) D4W_HC(12) D4W_HC(15) D4W_HC(16) D4W_HC(20) D4W_HC(25)
-#undef D4W_HC
-            default: return fail(D4W_ERR_UNSUPPORTED, "row split radix not built");
-        }
+        k_hsplit_inv2<T1><<<g, thr, 0, stream>>>(w, x, nx, p->ns, out, p->t2, p->d_twT, mode, dev_stats);
         D4W_CHECK_LAUNCH("k_hsplit_inv2");
         return D4W_OK;
-    }
-    float2* w = (float2*)workspace;
-    const int threads = 128;
-    dim3 grid((p->t2 + threads - 1) / threads, nx);
-    switch (p->t1) {
-#define D4W_HC(T) case T: k_hsplit_fwd<T><<<grid, threads, 0, stream>>>(x, p->ns, w, p->t2, p->d_twT); break;
-        D4W_HC(2) D4W_HC(3) D4W_HC(4) D4W_HC(5) D4W_HC(6) D4W_HC(8) D4W_HC(10) D4W_HC(12) D4W_HC(15) D4W_HC(16) D4W_HC(20) D4W_HC(25)
-#undef D4W_HC
-        default: return fail(D4W_ERR_UNSUPPORTED, "row split radix not built");
-    }
-    D4W_CHECK_LAUNCH("k_hsplit_fwd");
-    dim3 gmid(p->t1, nx);
-    if (p->fused) k_row_mid_fused<<<gmid, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->ns, p->d_hilbert, (size_t)0);
-    else k_row_mid<<<gmid, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->ns, p->d_hilbert, (size_t)0);
-    D4W_CHECK_LAUNCH("k_row_mid");
-    switch (p->t1) {
-#define D4W_HC(T) case T: k_hsplit_inv<T><<<grid, threads, 0, stream>>>(w, p->ns, out, p->t2, p->d_twT, mode, dev_stats); break;
-        D4W_HC(2) D4W_HC(3) D4W_HC(4) D4W_HC(5) D4W_HC(6) D4W_HC(8) D4W_HC(10) D4W_HC(12) D4W_HC(15) D4W_HC(16) D4W_HC(20) D4W_HC(25)
-#undef D4W_HC
-        default: return fail(D4W_ERR_UNSUPPORTED, "row split radix not built");
-    }
-    D4W_CHECK_LAUNCH("k_hsplit_inv");
-    return D4W_OK;
+    });
+    return rc == D4W_ERR_UNSUPPORTED ? fail(rc, "row split radix not built") : rc;
 }
 
 // ------------------------------------------------------------------ forward-backward SOS IIR
@@ -361,7 +317,7 @@ extern "C" int d4w_sosfiltfilt(const float* x, float* y, float* tmp, int nx, int
     }
     const int next = ns + 2 * padlen;
     int chunk = 0, warm = 0;
-    if (env_int("D4W_IIR_CHUNKED", 1) && rmax > 0.0 && rmax < 0.9995) {
+    if (rmax > 0.0 && rmax < 0.9995) {
         warm = (int)std::ceil(std::log(1e-9) / std::log(rmax)) + 32;
         warm = (warm + 31) / 32 * 32;
         chunk = std::max(4 * warm, 4096);
@@ -370,7 +326,7 @@ extern "C" int d4w_sosfiltfilt(const float* x, float* y, float* tmp, int nx, int
     }
     const int nchunks = chunk > 0 ? (next + chunk - 1) / chunk : 1;
     // four warps per block (one 32-channel group each); with time chunking every warp walks two chunks at once
-    const int nch = (nchunks >= 2 && env_int("D4W_IIR_NCH", 2) >= 2) ? 2 : 1;
+    const int nch = nchunks >= 2 ? 2 : 1;
     dim3 grid((blocks + 3) / 4, (nchunks + nch - 1) / nch);
 #define D4W_SOS(NS_, NCH_)                                                                               \
     do {                                                                                                 \
@@ -443,17 +399,13 @@ static int launch_stft_slide_g(d4w_fft_plan* p, const float* x, float* out, int 
 // runs per CTA: narrow bands take more runs so that runs x (bins + 2) threads fill the CTA
 template <int H, int P>
 static int launch_stft_slide(d4w_fft_plan* p, const float* x, float* out, int nx, const SlideParams& sp, cudaStream_t st) {
-    // measured on 1000 x 120 000 (scripts/gpu_slide_tune.py): 16 runs only pay below ~10 bins (0.69 vs 0.86 ms for 7 bins);
-    // at 13 bins their larger sample buffer forces shorter runs and loses (1.15 vs 0.94 ms)
-    int G = sp.nY <= 10 ? 16 : 8;
-    const int forced = env_int("D4W_SLIDE_G", 0);                 // tuning override; must keep G * nY <= 320
-    if ((forced == 8 || forced == 16) && forced * sp.nY <= kSlideMaxThreads) G = forced;
-    if (G == 16) return launch_stft_slide_g<H, P, 16>(p, x, out, nx, sp, st);
+    // measured on an H100 at 1000 x 120 000 (sweep of G and of the starting Q): 16 runs only pay below ~10 bins (0.69 vs
+    // 0.86 ms for 7 bins); at 13 bins their larger sample buffer forces shorter runs and loses (1.15 vs 0.94 ms)
+    if (sp.nY <= 10) return launch_stft_slide_g<H, P, 16>(p, x, out, nx, sp, st);
     return launch_stft_slide_g<H, P, 8>(p, x, out, nx, sp, st);
 }
 
 extern "C" int d4w_stft_slide_supported(int nfft, int hop, int nbins) {
-    if (!env_int("D4W_STFT_SLIDE", 1)) return 0;
     if (nbins < 1 || 8 * (nbins + 2) > kSlideMaxThreads) return 0;
     return (nfft == 160 && hop == 8) || (nfft == 128 && hop == 8) || (nfft == 256 && hop == 16);
 }
@@ -471,7 +423,7 @@ extern "C" int d4w_stft_slide(d4w_fft_plan* p, const float* x, float* out, int n
     SlideParams sp{};
     sp.ns = ns; sp.nframes = 1 + ns / hop; sp.nbins = nbins; sp.bin_lo = bin_lo;
     sp.nY = nbins + 2; sp.nYp = sp.nY | 1;                   // odd pitch: conflict-free 8-byte reads along frames
-    sp.Q = std::max(1, env_int("D4W_SLIDE_Q", 8));
+    sp.Q = 8;                                                // sub-steps per run; launch_stft_slide_g shrinks it to fit
     cudaStream_t st = (cudaStream_t)stream_v;
     if (p->n == 160) return launch_stft_slide<8, 20>(p, x, out, nx, sp, st);
     if (p->n == 128) return launch_stft_slide<8, 16>(p, x, out, nx, sp, st);
@@ -576,14 +528,13 @@ static int launch_speccorr_untiled(const float* S, int nx, int nfs, int nt, cons
 
 // All kernels in one k_speccorr4 pass when their tile fits; otherwise one pass per kernel, tiled or untiled.
 static int speccorr_kernels(const float* S, int nx, int nfs, int nt, const SpecKernel* ks, int nk, cudaStream_t st) {
-    const bool tiled = env_int("D4W_SPECCORR4", 1) != 0;
     SpecCorrSet set;
     size_t smem = speccorr4_set(ks, nk, nfs, set);
-    if (tiled && smem <= 110 * 1024) return launch_speccorr4(S, nx, nt, set, smem, st);
+    if (smem <= 110 * 1024) return launch_speccorr4(S, nx, nt, set, smem, st);
     for (int k = 0; k < nk; ++k) {
         smem = speccorr4_set(ks + k, 1, nfs, set);
-        const int rc = (tiled && smem <= 110 * 1024) ? launch_speccorr4(S, nx, nt, set, smem, st)
-                                                     : launch_speccorr_untiled(S, nx, nfs, nt, ks[k], st);
+        const int rc = smem <= 110 * 1024 ? launch_speccorr4(S, nx, nt, set, smem, st)
+                                          : launch_speccorr_untiled(S, nx, nfs, nt, ks[k], st);
         if (rc != D4W_OK) return rc;
     }
     return D4W_OK;

@@ -2,13 +2,13 @@
 // epilogues every Hilbert route shares.
 //
 // With c[t] = exp(-i pi (t^2 mod 2n) / n), a convolution length m >= 2n - 1 and bhat = FFT_m(conj c, wrapped) / m
-// (fk_hostplan.hpp: czt_tables), the analytic signal with scipy.signal.hilbert's weights h (h/n, or sgn/n when two real rows
-// share one complex transform) is
+// (fk_hostplan.hpp: czt_tables), the analytic signal with scipy.signal.hilbert's weights h (h/n on the whole-row route; sgn/n
+// on the split route, where two real rows share one complex transform) is
 //   1. u = x c for t < n, 0 for n <= t < m
 //   2. v = IFFT_m(FFT_m(u) bhat)                      -> X[f] = c[f] v[f]
 //   3. z[f] = (h[f]/n) v[f] for f < n, 0 for f >= n     (the chirps between the two DFTs cancel)
 //   4. w = IFFT_m(FFT_m(z) conj bhat)                 (c is even, so the second kernel's spectrum is conj bhat)
-//   5. a[t] = conj(c[t]) w[t] for t < n, then hilbert_epilogue / hilbert_epilogue2.
+//   5. a[t] = conj(c[t]) w[t] for t < n, then hilbert_epilogue (whole row) / hilbert_epilogue2 (split).
 // Whole-row route (m <= 16 384): one CTA runs the four m-point transforms in shared memory (body_hczt_row).  Split route
 // (m = T1 x T2): body_hczt_fwd -> k_row_mid(_fused)_c with bhat -> body_hczt_turn (inverse T1 split, step 3 and forward T1
 // split in registers: for a given t2 both splits touch the index set {t2 + j T2}) -> k_row_mid(_fused)_c with conj bhat ->
@@ -76,13 +76,13 @@ __host__ __device__ inline void body_hczt_row(const RowParams& rp, const HcztPar
     for (int i = tid; i < n; i += nthr) dst[i] = hilbert_epilogue(cmulc(smem[i], hp.chirp[i]), mode, var);
 }
 
-// ---- split route, step 1: forward radix-T1 split of u = x c (zero from n on); workspace row pr holds rows 2pr, 2pr+1 as
-// a + i b when hp.pair, else row pr
+// ---- split route (hp.pair), step 1: forward radix-T1 split of u = x c (zero from n on); workspace row pr holds rows 2pr,
+// 2pr+1 as a + i b
 template <int T1>
 __host__ __device__ inline void body_hczt_fwd(const HcztParams& hp, const float* __restrict__ x, float2* __restrict__ w, int pr, int t2) {
     const int n = hp.n, t2len = hp.t2;
-    const int ra = hp.pair ? 2 * pr : pr;
-    const bool has_b = hp.pair && ra + 1 < hp.nx;
+    const int ra = 2 * pr;
+    const bool has_b = ra + 1 < hp.nx;
     const float* sa = x + (size_t)ra * n;
     float2 v[T1];
     static_for<T1>([&](auto jc) {
@@ -131,8 +131,8 @@ __host__ __device__ inline void body_hczt_inv(const HcztParams& hp, const float2
     twiddle_powers<T1>(hp.twT[t2], p);
     static_for<T1>([&](auto jc) { constexpr int j = decltype(jc)::value; if constexpr (j > 0) v[j] = cmulc(v[j], p[j]); });
     DFT<T1, true>::run(v);
-    const size_t ra = hp.pair ? 2 * (size_t)pr : (size_t)pr;
-    const bool has_b = hp.pair && ra + 1 < (size_t)hp.nx;
+    const size_t ra = 2 * (size_t)pr;
+    const bool has_b = ra + 1 < (size_t)hp.nx;
     const bool need_var = mode == EPI_SNR || mode == EPI_ENVSTD;
     const float va = need_var ? (float)stats[4 * ra + 2] : 1.f;
     const float vb = (need_var && has_b) ? (float)stats[4 * (ra + 1) + 2] : 1.f;
@@ -143,12 +143,8 @@ __host__ __device__ inline void body_hczt_inv(const HcztParams& hp, const float2
         const int t = t2 + j * t2len;
         if (t < n) {
             const float2 z = cmulc(v[j], hp.chirp[t]);
-            if (!hp.pair) {
-                oa[t] = hilbert_epilogue(z, mode, va);
-            } else {
-                oa[t] = hilbert_epilogue2(xa[t], z.y, mode, va);
-                if (has_b) oa[(size_t)n + t] = hilbert_epilogue2(xa[(size_t)n + t], -z.x, mode, vb);
-            }
+            oa[t] = hilbert_epilogue2(xa[t], z.y, mode, va);
+            if (has_b) oa[(size_t)n + t] = hilbert_epilogue2(xa[(size_t)n + t], -z.x, mode, vb);
         }
     });
 }

@@ -620,47 +620,7 @@ k_xcorr_pfa(XcorrParams xp, const int* __restrict__ tpos, const float* __restric
 // ------------------------------------------------------------------ Hilbert envelope / SNR on the T1 x T2 row engine
 // EPI_* modes and hilbert_epilogue / hilbert_epilogue2: hilbert_czt.cuh (shared with the chirp-z rows)
 
-// forward split reading the REAL row (imag = 0) and writing the complex workspace
-template <int T1>
-static __global__ void __launch_bounds__(128)
-k_hsplit_fwd(const float* __restrict__ x, int ns, float2* __restrict__ w, int t2len, const float2* __restrict__ twT) {
-    const int t2 = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t2 >= t2len) return;
-    const size_t row = blockIdx.y;
-    const float* src = x + row * ns + t2;
-    float2 v[T1];
-    static_for<T1>([&](auto jc) { constexpr int j = decltype(jc)::value; v[j] = make_float2(src[(size_t)j * t2len], 0.f); });
-    float2 p[T1];
-    twiddle_powers<T1>(twT[t2], p);
-    DFT<T1, false>::run(v);
-    float2* dst = w + row * ns + t2;
-    static_for<T1>([&](auto jc) {
-        constexpr int j = decltype(jc)::value;
-        dst[(size_t)j * t2len] = (j > 0) ? cmul(v[j], p[j]) : v[j];
-    });
-}
-
-// inverse split reading the complex workspace and writing |z| or the envelope SNR
-template <int T1>
-static __global__ void __launch_bounds__(128)
-k_hsplit_inv(const float2* __restrict__ w, int ns, float* __restrict__ out, int t2len, const float2* __restrict__ twT, int mode,
-             const double* __restrict__ stats) {
-    const int t2 = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t2 >= t2len) return;
-    const size_t row = blockIdx.y;
-    const float2* src = w + row * ns + t2;
-    float2 v[T1];
-    static_for<T1>([&](auto jc) { constexpr int j = decltype(jc)::value; v[j] = src[(size_t)j * t2len]; });
-    float2 p[T1];
-    twiddle_powers<T1>(twT[t2], p);
-    static_for<T1>([&](auto jc) { constexpr int j = decltype(jc)::value; if constexpr (j > 0) v[j] = cmulc(v[j], p[j]); });
-    DFT<T1, true>::run(v);
-    const float var = (mode == EPI_SNR || mode == EPI_ENVSTD) ? (float)stats[4 * row + 2] : 1.f;
-    float* dst = out + row * ns + t2;
-    static_for<T1>([&](auto jc) { constexpr int j = decltype(jc)::value; dst[(size_t)j * t2len] = hilbert_epilogue(v[j], mode, var); });
-}
-
-// ---- two real rows per complex transform --------------------------------------------------------------------
+// ---- split rows: two real rows per complex transform ------------------------------------------------------------
 // The Hilbert transform is linear and maps real rows to real rows, so for z = a + i b one complex FFT -> (-i sgn f) -> IFFT
 // yields H(a) + i H(b): half the transforms and half the workspace traffic of the analytic-signal route.  The middle
 // pass multiplies by the real table sgn(f)/ns (0 at DC and Nyquist, scipy.signal.hilbert's h - 1); the factor -i is

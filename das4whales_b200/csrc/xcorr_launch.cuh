@@ -49,7 +49,7 @@ static int xcorr_launch(d4w_fft_plan* p, const float* x, int nx, int ns, int val
     }
     bool small_radices = true;
     for (int st = 0; st < p->pl.nstages; ++st) small_radices = small_radices && xcorr_dual_radix_ok(p->pl.radix[st]);
-    if (p->fused && p->pl.nstages >= 2 && small_radices && smem_dual <= 110 * 1024 && env_int("D4W_XCORR_DUAL", 1)) {
+    if (p->fused && p->pl.nstages >= 2 && small_radices && smem_dual <= 110 * 1024) {
         D4W_CUDA_TRY(cudaFuncSetAttribute(k_xcorr_dual<SAME>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
         dim3 gridd((xp.nseg + 3) / 4, nx);
         k_xcorr_dual<SAME><<<gridd, 256, smem_dual, (cudaStream_t)stream>>>(xp, x, (const float2*)dev_tabs, dev_stats, dev_segpre,

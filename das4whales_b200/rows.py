@@ -1,8 +1,6 @@
 """Per-channel (row) operators on the GPU: row statistics, overlap-save matched filter, Hilbert
 envelope / SNR, forward-backward SOS IIR, batched STFT.  Thin host wrappers over libd4w.so
 (csrc/rows_kernels.cuh); inputs are contiguous float32 CUDA tensors [nx, ns]."""
-import os as _os
-
 import numpy as np
 import scipy.signal as sp
 
@@ -101,7 +99,7 @@ def _pick_block(L, ns=0):
     2500 taps the longest template one pass can take -- detect.shift_xcorr cuts longer ones into pieces)."""
     def nseg(nb):
         return (ns + (nb - L)) // (nb - L + 1) if ns else 0
-    if L <= 2520 // 8 and nseg(2520) <= 512 and _os.environ.get("D4W_XCORR_PFA", "1") != "0":
+    if L <= 2520 // 8 and nseg(2520) <= 512:
         return 2520
     for nb, lmax in ((1250, 156), (2500, 312), (5000, 2500)):
         if L <= lmax and (nseg(nb) <= 512 or nb == 5000):   # row statistics keep at most 512 segment prefixes per row
@@ -365,23 +363,35 @@ def stft_mag(x, nfft, hop, bin_lo=0, bin_hi=None):
     torch = _torch()
     dev = _check_input(x)
     nx, ns = x.shape
-    plan = fft_plan(nfft, dev)
-    nframes = 1 + ns // hop
     bin_hi = nfft // 2 if bin_hi is None else int(bin_hi)
-    out = torch.empty((nx, bin_hi - bin_lo + 1, nframes), dtype=torch.float32, device=x.device)
+    L = _lib.lib()
+    if not L.d4w_stft_slide_supported(int(nfft), int(hop), bin_hi - bin_lo + 1):    # sliding DFT: band of bins, hop | n_fft
+        return _stft_frames(x, nfft, hop, bin_lo, bin_hi)
+    plan = fft_plan(nfft, dev)
+    out = torch.empty((nx, bin_hi - bin_lo + 1, 1 + ns // hop), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(dev):
+        for r0 in range(0, nx, 65535):
+            r1 = min(nx, r0 + 65535)
+            _lib.check(L.d4w_stft_slide(plan.ptr, _lib.ptr(x[r0:r1], "float*"), _lib.ptr(out[r0:r1], "float*"), r1 - r0, ns,
+                                        int(hop), int(bin_lo), bin_hi, _lib.stream_ptr()), "stft_slide")
+    return out
+
+
+def _stft_frames(x, nfft, hop, bin_lo, bin_hi):
+    """stft_mag by one FFT per frame (d4w_stft_mag), for the shapes the sliding DFT does not cover"""
+    torch = _torch()
+    dev = _check_input(x)
+    nx, ns = x.shape
+    plan = fft_plan(nfft, dev)
+    out = torch.empty((nx, bin_hi - bin_lo + 1, 1 + ns // hop), dtype=torch.float32, device=x.device)
     key = ("hann", nfft, dev)
     if key not in _tab_cache:
         _tab_cache[key] = torch.from_numpy(sp.get_window("hann", nfft, fftbins=True).astype(np.float32)).to(x.device)
     win = _tab_cache[key]
     L = _lib.lib()
-    slide = bool(L.d4w_stft_slide_supported(int(nfft), int(hop), bin_hi - bin_lo + 1))    # band of bins, hop | n_fft
     with torch.cuda.device(dev):
         for r0 in range(0, nx, 65535):
             r1 = min(nx, r0 + 65535)
-            if slide:
-                _lib.check(L.d4w_stft_slide(plan.ptr, _lib.ptr(x[r0:r1], "float*"), _lib.ptr(out[r0:r1], "float*"), r1 - r0, ns,
-                                            int(hop), int(bin_lo), bin_hi, _lib.stream_ptr()), "stft_slide")
-                continue
             _lib.check(L.d4w_stft_mag(plan.ptr, _lib.ptr(x[r0:r1], "float*"), _lib.ptr(out[r0:r1], "float*"), r1 - r0, ns,
                                       int(hop), _lib.ptr(win, "float*"), int(bin_lo), bin_hi, _lib.stream_ptr()), "stft_mag")
     return out

@@ -12,7 +12,7 @@ x = synth.synth_strain(NX, NS, seed=5)
 t = np.arange(NS) / FS
 tpls = [dw.detect.gen_template_fincall(t, FS, 17.8, 28.8, 0.68), dw.detect.gen_template_fincall(t, FS, 14.7, 21.8, 0.78)]
 hf, lf = dw.detect.compute_cross_correlograms(x, tpls)             # k_row_stats, k_xcorr
-env = rows.envelope(hf)                                            # k_hsplit_fwd, k_hilbert_row, k_hsplit_inv
+env = rows.envelope(hf)                                            # k_hsplit_fwd2, k_row_mid_fused, k_hsplit_inv2
 snr = dw.dsp.snr_tr_array(hf, env=True); snr2 = dw.dsp.snr_tr_array(hf, env=False)   # k_snr_plain
 bp = dw.dsp.bp_filt(x, FS, 14.0, 30.0)                             # k_sos_pass
 picks = rows.find_peaks_flags(env, 6.0)                            # k_peak_levels, k_peak_pick

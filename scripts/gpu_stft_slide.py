@@ -20,10 +20,8 @@ for (nfft, hop, b0, b1, ns) in [(160, 8, 2, 32, 9000), (160, 8, 0, 30, 9001), (1
     x = rng.standard_normal((5, ns)).astype(np.float32)
     x[1] += 50 * np.sin(2 * np.pi * 0.7 * np.arange(ns) / 200).astype(np.float32)
     xd = torch.from_numpy(x).cuda()
-    os.environ["D4W_STFT_SLIDE"] = "1"
     a = rows.stft_mag(xd, nfft, hop, b0, b1).cpu().numpy()
-    os.environ["D4W_STFT_SLIDE"] = "0"
-    b = rows.stft_mag(xd, nfft, hop, b0, b1).cpu().numpy()
+    b = rows._stft_frames(xd, nfft, hop, b0, b1).cpu().numpy()
     errs = []
     for i in range(5):
         ref = np.abs(O.stft_librosa(x[i].astype(np.float64), nfft, hop))[b0:b1 + 1]
@@ -33,23 +31,15 @@ for (nfft, hop, b0, b1, ns) in [(160, 8, 2, 32, 9000), (160, 8, 0, 30, 9001), (1
 nx, ns = 1000, 120000
 xd = synth.synth_strain(nx, ns, seed=3) if hasattr(synth, "synth_strain") else torch.randn(nx, ns, device="cuda")
 xd = xd.cuda() if not xd.is_cuda else xd
-os.environ["D4W_STFT_SLIDE"] = "0"
-t_fft = timed(lambda: rows.stft_mag(xd, 160, 8, 11, 41))
+t_fft = timed(lambda: rows._stft_frames(xd, 160, 8, 11, 41))
 print(f"fft path   {nx}x{ns} bins 11..41: {t_fft:.2f} ms -> {t_fft * 10:.1f} ms per 10 000 channels")
-os.environ["D4W_STFT_SLIDE"] = "1"
-for q in (2, 3, 4, 5, 6, 8):
-    os.environ["D4W_SLIDE_Q"] = str(q)
-    try:
-        t = timed(lambda: rows.stft_mag(xd, 160, 8, 11, 41))
-        print(f"slide Q={q}  {t:.2f} ms -> {t * 10:.1f} ms per 10 000 channels")
-    except Exception as e:
-        print("Q", q, "failed:", str(e)[:100])
-os.environ.pop("D4W_SLIDE_Q")
+t = timed(lambda: rows.stft_mag(xd, 160, 8, 11, 41))
+print(f"slide path {nx}x{ns} bins 11..41: {t:.2f} ms -> {t * 10:.1f} ms per 10 000 channels")
 kern = {'f0': 27., 'f1': 17., 'dur': 0.8, 'bdwidth': 4.}
 t = timed(lambda: dw.detect.compute_cross_correlogram_spectrocorr(xd, 200., [14., 30.], kern, 0.8, 0.95), reps=3)
 print(f"spectrocorr detector {nx} rows: {t:.2f} ms -> {t * 10:.1f} ms per 10 000 channels")
 
-# ---- median (sample-bracketed select) and register-tiled spectrogram correlation
+# ---- median (sample-bracketed select) and spectrogram correlation
 for name, a in [("rayleigh", np.abs(rng.standard_normal((7, 465031)) + 1j * rng.standard_normal((7, 465031)))),
                 ("even", rng.random((5, 200000))), ("ties", np.floor(rng.random((5, 300001)) * 7)),
                 ("half zeros", np.where(rng.random((4, 100001)) < 0.6, 0.0, rng.random((4, 100001)))),
@@ -59,22 +49,12 @@ for name, a in [("rayleigh", np.abs(rng.standard_normal((7, 465031)) + 1j * rng.
     got = rows.row_median(torch.from_numpy(a).cuda()).cpu().numpy()
     ref = np.median(a, axis=1)
     print(f"median {name:16s} n={a.shape[1]:7d}: exact={bool(np.array_equal(got, ref))}", flush=True)
-S = torch.from_numpy(np.abs(rng.standard_normal((3, 31, 15001))).astype(np.float32)).cuda()
-for kw in (19, 20, 21, 37):
-    Kk = rng.standard_normal((31, kw))
-    os.environ["D4W_SPECCORR4"] = "1"; o4 = rows.spectro_correlate(S, Kk)
-    os.environ["D4W_SPECCORR4"] = "0"; o1 = rows.spectro_correlate(S, Kk)
-    print(f"speccorr4 kw={kw}: bit-equal to untiled kernel = {bool(torch.equal(o4, o1))}")
-os.environ["D4W_SPECCORR4"] = "1"
 Sx = rows.stft_mag(xd, 160, 8, 11, 41)
 flat = Sx.reshape(nx, -1)
 t_med = timed(lambda: rows.row_median(flat))
 medv = rows.row_median(flat)
 Kk = rng.standard_normal((31, 20))
 t_sc = timed(lambda: rows.spectro_correlate(Sx, Kk, median=medv))
-os.environ["D4W_SPECCORR4"] = "0"
-t_sc1 = timed(lambda: rows.spectro_correlate(Sx, Kk, median=medv))
-os.environ["D4W_SPECCORR4"] = "1"
-print(f"row_median {nx} rows x {flat.shape[1]}: {t_med:.2f} ms; speccorr tiled {t_sc:.2f} ms, untiled {t_sc1:.2f} ms")
+print(f"row_median {nx} rows x {flat.shape[1]}: {t_med:.2f} ms; speccorr {t_sc:.2f} ms")
 t = timed(lambda: dw.detect.compute_cross_correlogram_spectrocorr(xd, 200., [14., 30.], kern, 0.8, 0.95), reps=3)
 print(f"spectrocorr detector {nx} rows: {t:.2f} ms -> {t * 10:.1f} ms per 10 000 channels")

@@ -1,6 +1,7 @@
 // CPU emulation of the chirp-z Hilbert rows (row lengths with no T1 x T2 split): runs the SAME __host__ __device__ bodies as
 // the GPU (hilbert_czt.cuh: body_hczt_row, or body_hczt_fwd -> body_row_mid(_fused) -> body_hczt_turn -> body_row_mid(_fused)
-// -> body_hczt_inv) with nthr = 1.  D4W_ROW_FUSED and D4W_HILBERT_PAIR select the route exactly as d4w_row_plan_create does.
+// -> body_hczt_inv) with nthr = 1.  D4W_ROW_FUSED selects the middle pass exactly as d4w_row_plan_create does; split rows
+// always take two real rows per transform.
 // usage:
 //   row_czt_emul plan N...          one line per N: "N direct T1 T2" | "N czt M T1 T2 fused" | "N error <message>"
 //   row_czt_emul tables N out.bin   int32 m, t1, t2, fused ; complex64 chirp[N] ; complex64 bhat[m] ; int32 tab2freq[m]
@@ -12,6 +13,7 @@
 #include <vector>
 #include "../../das4whales_b200/csrc/fk_hostplan.hpp"
 #include "../../das4whales_b200/csrc/hilbert_czt.cuh"
+#include "../../das4whales_b200/csrc/row_plan.hpp"
 using namespace d4w;
 
 static const size_t kSmem = 227 * 1024;
@@ -28,7 +30,7 @@ static std::vector<int> table_order(const RowCztPlan& cz) {
 template <int T1>
 static void split_route(const RowCztPlan& cz, HcztParams hz, const float* x, float* y, int mode, const double* stats) {
     const FkHostPlan& hp = cz.hp;
-    const int nrow = hz.pair ? (hz.nx + 1) / 2 : hz.nx;
+    const int nrow = (hz.nx + 1) / 2;
     std::vector<float2> w((size_t)nrow * cz.m, make_float2(-777.f, -777.f)), smem((size_t)hp.t2 + 16);
     std::vector<float2> bc(cz.bhat.size());
     for (size_t i = 0; i < bc.size(); ++i) bc[i] = make_float2(cz.bhat[i].x, -cz.bhat[i].y);
@@ -96,7 +98,7 @@ int main(int argc, char** argv) {
         }
         HcztParams hz{};
         hz.n = n; hz.m = cz.m; hz.t2 = cz.hp.t2; hz.nx = nrows; hz.invn = (float)(1.0 / n);
-        hz.pair = (cz.hp.t1 > 1 && env_int("D4W_HILBERT_PAIR", 1)) ? 1 : 0;
+        hz.pair = cz.hp.t1 > 1 ? 1 : 0;
         hz.chirp = cz.chirp.data(); hz.twT = cz.hp.twT.data();
         if (cz.hp.t1 == 1) {
             std::vector<float2> bc(cz.bhat.size()), smem((size_t)cz.m + 16);
@@ -105,13 +107,12 @@ int main(int argc, char** argv) {
             rp.pl = cz.hp.rowpl; rp.tw = cz.hp.tw_row.data(); rp.twT = cz.hp.twT.data(); rp.t1 = 1; rp.t2 = cz.m;
             for (int r = 0; r < nrows; ++r)
                 body_hczt_row(rp, hz, cz.bhat.data(), bc.data(), x.data(), y.data(), mode, stats.data(), r, 0, 1, smem.data());
-        } else {
-            switch (cz.hp.t1) {
-#define D4W_HC(T) case T: split_route<T>(cz, hz, x.data(), y.data(), mode, stats.data()); break;
-                D4W_HC(2) D4W_HC(3) D4W_HC(4) D4W_HC(5) D4W_HC(6) D4W_HC(8) D4W_HC(10) D4W_HC(12) D4W_HC(15) D4W_HC(16) D4W_HC(20) D4W_HC(25)
-#undef D4W_HC
-                default: fprintf(stderr, "split %d not built\n", cz.hp.t1); return 5;
-            }
+        } else if (with_t1(cz.hp.t1, [&](auto tc) {
+                       split_route<decltype(tc)::value>(cz, hz, x.data(), y.data(), mode, stats.data());
+                       return D4W_OK;
+                   }) != D4W_OK) {
+            fprintf(stderr, "split %d not built\n", cz.hp.t1);
+            return 5;
         }
         FILE* fo = fopen(argv[3], "wb");
         const int info[3] = {cz.m, cz.hp.t1, hz.pair};

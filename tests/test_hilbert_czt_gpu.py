@@ -1,6 +1,6 @@
 """GPU parity of the Hilbert family for row lengths with no T1 x T2 split (chirp-z rows, csrc/hilbert_czt.cuh): envelope,
 H(x), envelope / std, envelope SNR and instant_freq against the float64 oracle on every route (whole row in one CTA below
-16 384 convolution points, five split launches above; one or two real rows per transform; either middle-pass kernel), the
+16 384 convolution points, five split launches on two real rows per transform above; either middle-pass kernel), the
 spectrogram-correlation flow of scripts/main_spectrodetect.py on 1 501-frame correlograms, and the 128 000-sample limit."""
 import numpy as np
 import pytest
@@ -30,7 +30,7 @@ def dw():
 
 @pytest.fixture
 def fresh_plans(monkeypatch):
-    """Plans read D4W_ROW_FUSED / D4W_HILBERT_PAIR when they are created: start from an empty cache, free what was made."""
+    """Plans read D4W_ROW_FUSED when they are created: start from an empty cache, free what was made."""
     from das4whales_b200 import _lib, rows
     monkeypatch.setattr(rows, "_row_plans", {})
     yield rows
@@ -56,7 +56,6 @@ def test_hilbert_family_czt_lengths(dw, fresh_plans, monkeypatch, env):
     rows = fresh_plans
     for k, v in env.items():
         monkeypatch.setenv(k, v)
-    pair = env.get("D4W_HILBERT_PAIR", "1") != "0"
     import torch
     for i, n in enumerate(LENGTHS):
         nx = (1, 2, 3)[i % 3]
@@ -83,7 +82,7 @@ def test_hilbert_family_czt_lengths(dw, fresh_plans, monkeypatch, env):
         assert m >= 2 * n - 1 and t1 * t2 == m, (n, t1, t2, m)
         assert (t1 == 1) == (m <= 16384), (n, t1, m)
         ws = _lib.lib().d4w_row_workspace_bytes(plan.ptr, nx)
-        assert ws == (16 if t1 == 1 else ((nx + 1) // 2 if pair else nx) * m * 8), (n, ws)
+        assert ws == (16 if t1 == 1 else (nx + 1) // 2 * m * 8), (n, ws)
 
 
 def test_plan_info_direct_lengths_unchanged(dw, fresh_plans):

@@ -16,7 +16,7 @@ from conftest import ROOT
 NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 pytestmark = pytest.mark.skipif(not os.path.exists(NVCC), reason="nvcc not available")
 EMUL = os.path.join(ROOT, "tests", "host_emul")
-ROUTES = [{}, {"D4W_ROW_FUSED": "0"}, {"D4W_HILBERT_PAIR": "0"}, {"D4W_ROW_FUSED": "0", "D4W_HILBERT_PAIR": "0"}]
+ROUTES = [{}, {"D4W_ROW_FUSED": "0"}]
 
 
 def _compile(tmp_path_factory, name):
@@ -40,7 +40,7 @@ def _smooth5(n):
 
 
 def _env(extra):
-    env = {k: v for k, v in os.environ.items() if k not in ("D4W_ROW_FUSED", "D4W_HILBERT_PAIR", "D4W_T1")}
+    env = {k: v for k, v in os.environ.items() if k not in ("D4W_ROW_FUSED", "D4W_T1")}
     env.update(extra)
     return env
 
@@ -165,7 +165,7 @@ def test_bodies_vs_scipy_hilbert(exe, tmp_path, n, extra):
         refs = {0: np.abs(a), 2: a.imag, 3: np.abs(a) / np.sqrt(var)}
         for mode, ref in refs.items():
             m, t1, pair, y = _run(exe, str(tmp_path), x, mode, extra)
-            assert (t1 == 1) == (n < 8192) and pair == (t1 > 1 and extra.get("D4W_HILBERT_PAIR", "1") != "0")
+            assert (t1 == 1) == (n < 8192) and pair == (t1 > 1)
             e = np.max(np.abs(y - ref)) / np.max(np.abs(ref))
             assert e <= 2e-6, (n, nrows, mode, e)
         _, _, _, y = _run(exe, str(tmp_path), x, 1, extra)

@@ -52,6 +52,34 @@ def test_cross_correlogram_vs_oracle(dw, nx, ns):
         assert e[0] <= 2e-5 and e[1] <= 2e-5, e
 
 
+def test_xcorr_unfused_block_plan(dw):
+    """k_xcorr, the overlap-save kernel for a block plan whose first or last radix is not register-resident (every plan of
+    1274 = 2 * 7^2 * 13 samples has 7, 13 or 14 at one end; _pick_block's lengths never do): d4w_xcorr through the ABI with
+    two templates, tables in plan.tab2freq order as cross_correlogram builds them, against float64 SciPy."""
+    import scipy.signal as sps
+    import torch
+    from das4whales_b200 import _lib, rows
+    nb, nx, ns = 1274, 3, 5000
+    plan = rows.fft_plan(nb, 0)
+    assert np.array_equal(plan.tab2freq, plan.pos2freq)         # no fused table order: neither k_xcorr_fused nor k_xcorr_dual
+    rng = np.random.default_rng(nb)
+    x = rng.standard_normal((nx, ns)).astype(np.float32)
+    taps = [rng.standard_normal(300), np.hanning(201) * np.sin(0.3 * np.arange(201))]
+    valid = nb - max(len(c) for c in taps) + 1
+    tabs = np.stack([(np.conj(np.fft.fft(c, nb)) / nb)[plan.tab2freq] for c in taps]).astype(np.complex64)
+    xd = torch.from_numpy(x).cuda()
+    tabs_d = torch.from_numpy(tabs.view(np.float32).reshape(len(taps), nb, 2)).cuda()
+    out = torch.empty((len(taps), nx, ns), dtype=torch.float32, device=xd.device)
+    null = _lib.ffi.NULL
+    _lib.check(_lib.lib().d4w_xcorr(plan.ptr, _lib.ptr(xd, "float*"), nx, ns, valid, len(taps), _lib.ptr(tabs_d), null, null,
+                                    null, _lib.ptr(out, "float*"), _lib.stream_ptr()), "xcorr")
+    got = out.cpu().numpy()
+    for i, c in enumerate(taps):
+        ref = sps.correlate(x.astype(np.float64), c[None, :], mode="full")[:, len(c) - 1:len(c) - 1 + ns]   # sum_n x[t+n] c[n]
+        e = rel_err(got[i], ref)
+        assert e[0] <= 1e-4 and e[1] <= 1e-5, (i, e)
+
+
 def test_envelope_and_picks_golden(dw, golden):
     g = golden("matched_filter")
     for tag in ("hf", "lf"):
@@ -77,17 +105,17 @@ def test_snr_golden_and_kat(dw, golden):
         assert rel_err(lin, lref)[0] <= TOL, env
 
 
-HILBERT_ROUTES = [{}, {"D4W_ROW_FUSED": "0"}, {"D4W_HILBERT_PAIR": "0"}, {"D4W_ROW_FUSED": "0", "D4W_HILBERT_PAIR": "0"}]
+HILBERT_ROUTES = [{}, {"D4W_ROW_FUSED": "0"}]
 
 
 @pytest.mark.parametrize("env", HILBERT_ROUTES)
 def test_envelope_routes_agree(dw, monkeypatch, env):
-    """Every route of the split-row Hilbert transform (two real rows per complex transform or one per row; middle pass
-    k_row_mid_fused, the default here, or k_row_mid) gives the oracle's envelope and SNR, an odd row count included."""
+    """Both middle passes of the split-row Hilbert transform (two real rows per complex transform; k_row_mid_fused, the
+    default here, or k_row_mid) give the oracle's envelope and SNR, an odd row count (a half-empty last pair) included."""
     from das4whales_b200 import _lib, rows
     for k, v in env.items():
         monkeypatch.setenv(k, v)
-    monkeypatch.setattr(rows, "_row_plans", {})                  # plans read the options when they are created
+    monkeypatch.setattr(rows, "_row_plans", {})                  # plans read D4W_ROW_FUSED when they are created
     nx, ns = 5, 120000
     x = np.random.default_rng(11).standard_normal((nx, ns)).astype(np.float32)
     L = _lib.lib()
@@ -99,8 +127,7 @@ def test_envelope_routes_agree(dw, monkeypatch, env):
     finally:
         for p in rows._row_plans.values():
             L.d4w_row_plan_destroy(p.ptr)
-    pair = env.get("D4W_HILBERT_PAIR", "1") != "0"
-    assert ws == ((nx + 1) // 2 if pair else nx) * ns * 8
+    assert ws == (nx + 1) // 2 * ns * 8
     assert rel_err(env_, D.envelope(x.astype(np.float64)))[0] <= 2e-5
     ref = O.snr_tr_array(x.astype(np.float64), env=True)
     assert rel_err(10 ** (snr / 10), 10 ** (ref / 10))[0] <= TOL
@@ -226,7 +253,6 @@ def test_stft_sliding_dft_band(dw, nfft, hop, b0, b1, ns):
     """d4w_stft_slide (sliding DFT over a band of bins) vs the fp64 restatement of librosa.stft and vs the per-frame FFT
     kernel; row 1 carries a strong out-of-band tone (the rectangular-window recursion sees its leakage, the Hann
     combination has to cancel it)."""
-    import os
     import torch
     from das4whales_b200 import rows, _lib
     assert _lib.lib().d4w_stft_slide_supported(nfft, hop, b1 - b0 + 1) == 1
@@ -236,11 +262,7 @@ def test_stft_sliding_dft_band(dw, nfft, hop, b0, b1, ns):
     x[2] += 1000.0                                                          # DC offset
     xd = torch.from_numpy(x).cuda()
     got = rows.stft_mag(xd, nfft, hop, b0, b1).cpu().numpy()
-    os.environ["D4W_STFT_SLIDE"] = "0"
-    try:
-        fft_path = rows.stft_mag(xd, nfft, hop, b0, b1).cpu().numpy()
-    finally:
-        del os.environ["D4W_STFT_SLIDE"]
+    fft_path = rows._stft_frames(xd, nfft, hop, b0, b1).cpu().numpy()
     assert got.shape == fft_path.shape == (4, b1 - b0 + 1, 1 + ns // hop)
     for i in range(4):
         full = np.abs(O.stft_librosa(x[i].astype(np.float64), nfft, hop))
