@@ -17,6 +17,10 @@ using namespace d4w;
 namespace d4w {
 std::string& last_error_ref() { static thread_local std::string e; return e; }
 std::atomic<long long>& launch_counter() { static std::atomic<long long> c{0}; return c; }
+// mask-bank kernels (d4w_fk_bank.cu)
+int launch_row_mid_oop(bool dual, bool fused, dim3 grid, int threads, size_t smem, const RowParams& rp, float2* w, size_t ldw,
+                       const float* tab, size_t tab_slot_stride, int nslots, float2* dst, int device, cudaStream_t stream);
+int launch_bank_gather(const float* src, float* dst, const int* src_row, int ns, size_t total, cudaStream_t stream);
 }  // namespace d4w
 
 extern "C" const char* d4w_last_error(void) { return last_error_ref().c_str(); }
@@ -239,6 +243,8 @@ extern "C" int d4w_fk_plan_info(const d4w_fk_plan* pl, int* info) {
 }
 
 // ------------------------------------------------------------------------------- masks
+static int build_support_tables(d4w_fk_mask* m, const std::vector<int>& act_k);
+
 // eps_arg < 0: exact pruning unless the environment variable D4W_MASK_EPS says otherwise
 static int mask_finish_support(d4w_fk_mask* m, void* stream_v, double eps_arg = -1.0) {
     d4w_fk_plan* pl = m->plan;
@@ -262,14 +268,24 @@ static int mask_finish_support(d4w_fk_mask* m, void* stream_v, double eps_arg = 
     // exact pruning by default; D4W_MASK_EPS > 0 additionally drops rows whose folded mask never exceeds eps
     const char* eps_s = std::getenv("D4W_MASK_EPS");
     const float eps = eps_arg >= 0.0 ? (float)eps_arg : (eps_s && *eps_s) ? (float)std::atof(eps_s) : 0.0f;
+    std::vector<int> act_k;
+    for (int k = 0; k < nrows; ++k) {
+        float v; std::memcpy(&v, &rowmax[k], 4);
+        if (v > eps) act_k.push_back(k);
+    }
+    return build_support_tables(m, act_k);
+}
+
+// Per-slot column tables for the kept wavenumber rows act_k (ascending, in [0, nx/2]): slot positions, the two-level
+// plane entries and need tables.  Used for a mask's own support and for the union support of a mask bank.
+static int build_support_tables(d4w_fk_mask* m, const std::vector<int>& act_k) {
+    d4w_fk_plan* pl = m->plan;
+    const int nrows = pl->nx / 2 + 1;
     cudaFree(m->d_act_k); cudaFree(m->d_k2slot); cudaFree(m->d_slot_pos); cudaFree(m->d_plane_ptr); cudaFree(m->d_ents); cudaFree(m->d_need);
     m->d_act_k = m->d_k2slot = nullptr; m->d_slot_pos = nullptr; m->d_plane_ptr = nullptr; m->d_ents = nullptr; m->d_need = nullptr;
     std::vector<int> k2slot((size_t)nrows, -1);
-    m->act_k.clear();
-    for (int k = 0; k < nrows; ++k) {
-        float v; std::memcpy(&v, &rowmax[k], 4);
-        if (v > eps) { k2slot[k] = (int)m->act_k.size(); m->act_k.push_back(k); }
-    }
+    m->act_k = act_k;
+    for (size_t sl = 0; sl < act_k.size(); ++sl) k2slot[act_k[sl]] = (int)sl;
     m->nact = (int)m->act_k.size();
     D4W_CUDA_TRY(upload(&m->d_act_k, m->act_k));
     D4W_CUDA_TRY(upload(&m->d_k2slot, k2slot));
@@ -393,16 +409,24 @@ extern "C" int d4w_fk_mask_materialize(const d4w_fk_mask* m, double* dev_out, vo
 }
 
 // ------------------------------------------------------------------------------- apply
+// bytes of one block of kept rows W (|support| x ns complex samples), rounded up so that what follows stays aligned
+static size_t kept_rows_bytes(const d4w_fk_plan* pl, int nact) {
+    const size_t b = std::max<size_t>((size_t)nact * pl->ns * sizeof(float2), 16);
+    return (b + 255) / 256 * 256;
+}
+
+// bytes of the level-A/B intermediate V of a two-level plan (chunk ring and its counters), 0 for other plans
+static size_t col2_ring_bytes(const d4w_fk_plan* pl) {
+    if (!pl->two_level) return 0;
+    const int nbuf = pl->pipe.nchunks ? pl->pipe.nbuf : 1;
+    size_t b = (size_t)nbuf * pl->col2.planes * pl->col2.x2 * pl->col2.vhp * sizeof(cpd);     // level-A/B intermediate V (chunk ring)
+    if (pl->pipe.nchunks) b += (size_t)(2 * pl->pipe.nchunks + 1 + 63) / 64 * 64 * sizeof(unsigned);   // ticket + chunk counters
+    return b;
+}
+
 extern "C" size_t d4w_fk_workspace_bytes(const d4w_fk_plan* pl, const d4w_fk_mask* m) {
     if (!pl || !m) return 0;
-    size_t b = std::max<size_t>((size_t)m->nact * pl->ns * sizeof(float2), 16);
-    b = (b + 255) / 256 * 256;
-    if (pl->two_level) {
-        const int nbuf = pl->pipe.nchunks ? pl->pipe.nbuf : 1;
-        b += (size_t)nbuf * pl->col2.planes * pl->col2.x2 * pl->col2.vhp * sizeof(cpd);     // level-A/B intermediate V (chunk ring)
-        if (pl->pipe.nchunks) b += (size_t)(2 * pl->pipe.nchunks + 1 + 63) / 64 * 64 * sizeof(unsigned);   // ticket + chunk counters
-    }
-    return b;
+    return kept_rows_bytes(pl, m->nact) + col2_ring_bytes(pl);
 }
 
 template <bool INV>
@@ -504,39 +528,17 @@ static int launch_col2_pipe(const d4w_fk_plan* pl, const d4w_fk_mask* m, const f
     return D4W_OK;
 }
 
-extern "C" int d4w_fk_apply_pass_ex(d4w_fk_plan* pl, d4w_fk_mask* m, const float* x, float* y, void* ws, int taper,
-                                    int pass, int slot_begin, int slot_count, int t_offset, void* stream_v) {
-    if (!pl || !m || !ws) return fail(D4W_ERR_ARG, "d4w_fk_apply: null argument");
-    d4w_fk_plan* mp = m->plan;
-    if (!m->d_table) return fail(D4W_ERR_ARG, "d4w_fk_apply: call d4w_fk_mask_build first");
-    if (pl->device != mp->device) return fail(D4W_ERR_ARG, "d4w_fk_apply: plan and mask live on different devices");
-    DeviceGuard guard(pl->device);
-    cudaStream_t stream = (cudaStream_t)stream_v;
-    float2* w = (float2*)ws;
+// One pass on explicit buffers, arguments already checked.  w: the kept rows of m's support; v2: the two-level
+// intermediate (nullptr: the single-level column kernels); tab: P3's table for the `slot_count` rows at w; w3: P3's
+// destination (nullptr: in place, the single-mask filter; otherwise a second kept-row block of the same layout).
+static int fk_run_pass(const d4w_fk_plan* pl, const d4w_fk_mask* m, const float* x, float* y, float2* w, cpd* v2,
+                       const float* tab, float2* w3, const float* tap, int pass, int slot_count, cudaStream_t stream) {
+    const d4w_fk_plan* mp = m->plan;
     const size_t ldw = (size_t)pl->ns;
     const int nact = m->nact;
-    if (pass == 1 || pass == 5) {
-        if (pl->nx != mp->nx) return fail(D4W_ERR_ARG, "d4w_fk_apply: column passes need the mask's channel count");
-        if (t_offset < 0 || (long long)t_offset + pl->ns > mp->ns) return fail(D4W_ERR_ARG, "d4w_fk_apply: time slab outside the mask's time axis");
-    } else {
-        if (pl->ns != mp->ns) return fail(D4W_ERR_ARG, "d4w_fk_apply: time passes need the mask's full time axis");
-        if (slot_begin < 0 || slot_count < 0 || slot_begin + slot_count > nact) return fail(D4W_ERR_ARG, "d4w_fk_apply: bad slot range");
-    }
     const int tile = pl->col.dual ? 4 * pl->col.npair : 2 * pl->col.nc;
     const int ntiles = (pl->ns + tile - 1) / tile;
-    const float* tap = taper ? mp->d_taper + t_offset : nullptr;
-    // the per-plane tables of the mask were built for its own plan; a time-slab plan of the same channel axis has the very
-    // same two-level split (it depends on nx only), so the slab runs the two-level / pipelined kernels as well
-    const bool same_split = pl == mp || (pl->nx == mp->nx && pl->two_level && mp->two_level && pl->col2.x1 == mp->col2.x1 &&
-                                         pl->col2.x2 == mp->col2.x2 && pl->hostplan.fused_ra == mp->hostplan.fused_ra &&
-                                         pl->hostplan.fused_rb == mp->hostplan.fused_rb && pl->hostplan.pos_x2 == mp->hostplan.pos_x2);
-    const bool two = pl->two_level && same_split && m->d_ents && ((uintptr_t)ws % 16 == 0);
-    cpd* v2 = nullptr;
-    if (two) {
-        size_t wb = std::max<size_t>((size_t)nact * pl->ns * sizeof(float2), 16);
-        wb = (wb + 255) / 256 * 256;
-        v2 = reinterpret_cast<cpd*>(reinterpret_cast<char*>(ws) + wb);
-    }
+    const bool two = v2 != nullptr;
     switch (pass) {
         case 1:
             if (!x) return fail(D4W_ERR_ARG, "d4w_fk_apply: null input");
@@ -604,18 +606,20 @@ extern "C" int d4w_fk_apply_pass_ex(d4w_fk_plan* pl, d4w_fk_mask* m, const float
             if (slot_count == 0) return D4W_OK;
             if (pl->row.dual) {
                 dim3 grid(pl->t1, (slot_count + 1) / 2);
-                k_row_mid_dual<<<grid, env_int("D4W_ROW_DUAL_THREADS", 128), pl->row_smem, stream>>>(pl->row, w, ldw, m->d_table + (size_t)slot_begin * pl->ns,
-                                                                    (size_t)pl->ns, slot_count);
+                const int threads = env_int("D4W_ROW_DUAL_THREADS", 128);
+                if (w3) return launch_row_mid_oop(true, false, grid, threads, pl->row_smem, pl->row, w, ldw, tab, (size_t)pl->ns,
+                                                  slot_count, w3, pl->device, stream);
+                k_row_mid_dual<<<grid, threads, pl->row_smem, stream>>>(pl->row, w, ldw, tab, (size_t)pl->ns, slot_count);
                 D4W_CHECK_LAUNCH("k_row_mid_dual");
                 return D4W_OK;
             }
             dim3 grid(pl->t1, slot_count);
+            if (w3) return launch_row_mid_oop(false, pl->hostplan.row_fused, grid, pl->row_threads, pl->row_smem, pl->row, w, ldw,
+                                              tab, (size_t)pl->ns, slot_count, w3, pl->device, stream);
             if (pl->hostplan.row_fused)
-                k_row_mid_fused<<<grid, pl->row_threads, pl->row_smem, stream>>>(pl->row, w, ldw, m->d_table + (size_t)slot_begin * pl->ns,
-                                                                                 (size_t)pl->ns);
+                k_row_mid_fused<<<grid, pl->row_threads, pl->row_smem, stream>>>(pl->row, w, ldw, tab, (size_t)pl->ns);
             else
-                k_row_mid<<<grid, pl->row_threads, pl->row_smem, stream>>>(pl->row, w, ldw, m->d_table + (size_t)slot_begin * pl->ns,
-                                                                           (size_t)pl->ns);
+                k_row_mid<<<grid, pl->row_threads, pl->row_smem, stream>>>(pl->row, w, ldw, tab, (size_t)pl->ns);
             D4W_CHECK_LAUNCH("k_row_mid");
             return D4W_OK;
         }
@@ -685,6 +689,37 @@ extern "C" int d4w_fk_apply_pass_ex(d4w_fk_plan* pl, d4w_fk_mask* m, const float
     }
 }
 
+// the two-level kernels need their per-plane tables built for this channel split, and a 16-byte aligned workspace
+static bool use_two_level(const d4w_fk_plan* pl, const d4w_fk_mask* m, const void* ws) {
+    const d4w_fk_plan* mp = m->plan;
+    // the per-plane tables of the mask were built for its own plan; a time-slab plan of the same channel axis has the very
+    // same two-level split (it depends on nx only), so the slab runs the two-level / pipelined kernels as well
+    const bool same_split = pl == mp || (pl->nx == mp->nx && pl->two_level && mp->two_level && pl->col2.x1 == mp->col2.x1 &&
+                                         pl->col2.x2 == mp->col2.x2 && pl->hostplan.fused_ra == mp->hostplan.fused_ra &&
+                                         pl->hostplan.fused_rb == mp->hostplan.fused_rb && pl->hostplan.pos_x2 == mp->hostplan.pos_x2);
+    return pl->two_level && same_split && m->d_ents && ((uintptr_t)ws % 16 == 0);
+}
+
+extern "C" int d4w_fk_apply_pass_ex(d4w_fk_plan* pl, d4w_fk_mask* m, const float* x, float* y, void* ws, int taper,
+                                    int pass, int slot_begin, int slot_count, int t_offset, void* stream_v) {
+    if (!pl || !m || !ws) return fail(D4W_ERR_ARG, "d4w_fk_apply: null argument");
+    d4w_fk_plan* mp = m->plan;
+    if (!m->d_table) return fail(D4W_ERR_ARG, "d4w_fk_apply: call d4w_fk_mask_build first");
+    if (pl->device != mp->device) return fail(D4W_ERR_ARG, "d4w_fk_apply: plan and mask live on different devices");
+    DeviceGuard guard(pl->device);
+    if (pass == 1 || pass == 5) {
+        if (pl->nx != mp->nx) return fail(D4W_ERR_ARG, "d4w_fk_apply: column passes need the mask's channel count");
+        if (t_offset < 0 || (long long)t_offset + pl->ns > mp->ns) return fail(D4W_ERR_ARG, "d4w_fk_apply: time slab outside the mask's time axis");
+    } else {
+        if (pl->ns != mp->ns) return fail(D4W_ERR_ARG, "d4w_fk_apply: time passes need the mask's full time axis");
+        if (slot_begin < 0 || slot_count < 0 || slot_begin + slot_count > m->nact) return fail(D4W_ERR_ARG, "d4w_fk_apply: bad slot range");
+    }
+    const float* tap = taper ? mp->d_taper + t_offset : nullptr;
+    cpd* v2 = use_two_level(pl, m, ws) ? reinterpret_cast<cpd*>(reinterpret_cast<char*>(ws) + kept_rows_bytes(pl, m->nact)) : nullptr;
+    return fk_run_pass(pl, m, x, y, (float2*)ws, v2, m->d_table + (size_t)slot_begin * pl->ns, nullptr, tap, pass, slot_count,
+                       (cudaStream_t)stream_v);
+}
+
 extern "C" int d4w_fk_apply_pass(d4w_fk_plan* pl, d4w_fk_mask* m, const float* x, float* y, void* ws, int taper,
                                  int pass, void* stream) {
     if (!pl || !m) return fail(D4W_ERR_ARG, "d4w_fk_apply: null argument");
@@ -699,4 +734,142 @@ extern "C" int d4w_fk_apply(d4w_fk_plan* pl, d4w_fk_mask* m, const float* x, flo
         if (rc != D4W_OK) return rc;
     }
     return D4W_OK;
+}
+
+// ------------------------------------------------------------------------------- mask banks
+// Several masks over one plan and one forward transform (scripts/main_fkcomp.py:66-95 filters the same band-passed
+// matrix with four masks).  The bank's slots are the union U of the masks' kept rows in ascending wavenumber order,
+// so P1, P2 and P4 and the kept-row layout are those of a mask with support U.  Each mask gets a [|U|][ns] table
+// holding its own table's rows at its own slots and exact zeros elsewhere, which keeps a mask's arithmetic on every
+// row it keeps and leaves the rows it drops at zero.
+struct d4w_fk_bank {
+    d4w_fk_plan* plan = nullptr;
+    std::vector<d4w_fk_mask*> masks;
+    std::vector<std::vector<int>> supports;   // each mask's kept rows when the bank was made
+    d4w_fk_mask* sup = nullptr;               // the union support: its slot and column tables (no mask table)
+    int* d_src_row = nullptr;                 // [nmasks][|U|]: row of mask i's own table for slot u, -1 where it keeps none
+    float* d_table = nullptr;                 // caller-owned [nmasks][|U|][ns], set by d4w_fk_bank_build
+};
+
+extern "C" int d4w_fk_bank_destroy(d4w_fk_bank* b) {
+    if (!b) return D4W_OK;
+    DeviceGuard guard(b->plan->device);
+    d4w_fk_mask_destroy(b->sup);
+    cudaFree(b->d_src_row);
+    delete b;
+    return D4W_OK;
+}
+
+extern "C" int d4w_fk_bank_create(d4w_fk_bank** out, d4w_fk_plan* plan, d4w_fk_mask* const* masks, int nmasks) {
+    if (!out) return fail(D4W_ERR_ARG, "d4w_fk_bank_create: null output pointer");
+    *out = nullptr;
+    if (!plan || !masks) return fail(D4W_ERR_ARG, "d4w_fk_bank_create: null argument");
+    if (nmasks < 1) return fail(D4W_ERR_ARG, "d4w_fk_bank_create: a bank needs at least one mask");
+    for (int i = 0; i < nmasks; ++i) {
+        if (!masks[i]) return fail(D4W_ERR_ARG, "d4w_fk_bank_create: null mask " + std::to_string(i));
+        if (masks[i]->plan != plan) return fail(D4W_ERR_ARG, "d4w_fk_bank_create: mask " + std::to_string(i) + " was built for another plan");
+    }
+    DeviceGuard guard(plan->device);
+    const int nrows = plan->nx / 2 + 1;
+    std::vector<char> kept((size_t)nrows, 0);
+    for (int i = 0; i < nmasks; ++i)
+        for (int k : masks[i]->act_k) kept[k] = 1;
+    std::vector<int> uni;
+    for (int k = 0; k < nrows; ++k)
+        if (kept[k]) uni.push_back(k);
+    auto b = new d4w_fk_bank();
+    b->plan = plan;
+    b->masks.assign(masks, masks + nmasks);
+    b->sup = new d4w_fk_mask();
+    b->sup->plan = plan; b->sup->device = plan->device;
+    int rc = build_support_tables(b->sup, uni);
+    if (rc != D4W_OK) { d4w_fk_bank_destroy(b); return rc; }
+    const size_t nu = uni.size();
+    std::vector<int> src_row((size_t)nmasks * nu, -1);
+    for (int i = 0; i < nmasks; ++i) {
+        const std::vector<int>& s = masks[i]->act_k;
+        b->supports.push_back(s);
+        size_t j = 0;                                   // both lists ascend, and s is a subset of uni
+        for (size_t u = 0; u < nu && j < s.size(); ++u)
+            if (uni[u] == s[j]) src_row[(size_t)i * nu + u] = (int)j++;
+    }
+    cudaError_t e = upload(&b->d_src_row, src_row);
+    if (e != cudaSuccess) { d4w_fk_bank_destroy(b); return fail(D4W_ERR_CUDA, std::string("bank row map: ") + cudaGetErrorString(e)); }
+    *out = b;
+    return D4W_OK;
+}
+
+extern "C" int d4w_fk_bank_rows(const d4w_fk_bank* b) { return b ? b->sup->nact : 0; }
+
+extern "C" size_t d4w_fk_bank_table_bytes(const d4w_fk_bank* b) {
+    if (!b) return 0;
+    return std::max<size_t>(b->masks.size() * (size_t)b->sup->nact * b->plan->ns * sizeof(float), 16);
+}
+
+extern "C" int d4w_fk_bank_build(d4w_fk_bank* b, float* dev_table, void* stream_v) {
+    if (!b || !dev_table) return fail(D4W_ERR_ARG, "d4w_fk_bank_build: null argument");
+    DeviceGuard guard(b->plan->device);
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    for (size_t i = 0; i < b->masks.size(); ++i) {
+        const d4w_fk_mask* m = b->masks[i];
+        if (m->act_k != b->supports[i])
+            return fail(D4W_ERR_ARG, "d4w_fk_bank_build: mask " + std::to_string(i) + " was pruned again after the bank was made");
+        if (!m->d_table) return fail(D4W_ERR_ARG, "d4w_fk_bank_build: call d4w_fk_mask_build on mask " + std::to_string(i) + " first");
+    }
+    const int nu = b->sup->nact, ns = b->plan->ns;
+    const size_t total = (size_t)nu * ns;
+    for (size_t i = 0; i < b->masks.size() && total; ++i) {
+        const int rc = launch_bank_gather(b->masks[i]->d_table, dev_table + i * total, b->d_src_row + i * nu, ns, total, stream);
+        if (rc != D4W_OK) return rc;
+    }
+    b->d_table = dev_table;
+    return D4W_OK;
+}
+
+extern "C" size_t d4w_fk_bank_workspace_bytes(const d4w_fk_plan* pl, const d4w_fk_bank* b) {
+    if (!pl || !b) return 0;
+    return 2 * kept_rows_bytes(pl, b->sup->nact) + col2_ring_bytes(pl);
+}
+
+extern "C" int d4w_fk_bank_apply_pass(d4w_fk_plan* pl, d4w_fk_bank* b, const float* x, float* const* ys, void* ws, int taper,
+                                      int pass, int mask, void* stream_v) {
+    if (!pl || !b || !ys || !ws) return fail(D4W_ERR_ARG, "d4w_fk_bank_apply: null argument");
+    if (b->plan != pl) return fail(D4W_ERR_ARG, "d4w_fk_bank_apply: bank was built for a different plan");
+    if (!b->d_table) return fail(D4W_ERR_ARG, "d4w_fk_bank_apply: call d4w_fk_bank_build first");
+    const int nm = (int)b->masks.size();
+    if (pass >= 3 && (mask < 0 || mask >= nm)) return fail(D4W_ERR_ARG, "d4w_fk_bank_apply: mask index out of range");
+    // each output is written by its own P5 while the other masks still run, so no two outputs may overlap; an output
+    // may alias x, which is last read in P1
+    const size_t bytes = (size_t)pl->nx * pl->ns * sizeof(float);
+    for (int i = 0; i < nm; ++i) {
+        if (!ys[i]) return fail(D4W_ERR_ARG, "d4w_fk_bank_apply: null output " + std::to_string(i));
+        for (int j = 0; j < i; ++j) {
+            const char *a = (const char*)ys[i], *c = (const char*)ys[j];
+            if (a < c + bytes && c < a + bytes) return fail(D4W_ERR_ARG, "d4w_fk_bank_apply: outputs " + std::to_string(j) + " and " + std::to_string(i) + " overlap");
+        }
+    }
+    DeviceGuard guard(pl->device);
+    const d4w_fk_mask* sup = b->sup;
+    const int nu = sup->nact;
+    float2* w = (float2*)ws;                                                          // W: the forward transform
+    float2* w3 = (float2*)((char*)ws + kept_rows_bytes(pl, nu));                      // W': one mask's filtered rows
+    cpd* v2 = use_two_level(pl, sup, ws) ? reinterpret_cast<cpd*>((char*)ws + 2 * kept_rows_bytes(pl, nu)) : nullptr;
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    switch (pass) {
+        case 1: return fk_run_pass(pl, sup, x, nullptr, w, v2, nullptr, nullptr, taper ? pl->d_taper : nullptr, 1, nu, stream);
+        case 2: return fk_run_pass(pl, sup, nullptr, nullptr, w, v2, nullptr, nullptr, nullptr, 2, nu, stream);
+        case 3: return fk_run_pass(pl, sup, nullptr, nullptr, w, v2, b->d_table + (size_t)mask * nu * pl->ns, w3, nullptr, 3, nu, stream);
+        case 4: return fk_run_pass(pl, sup, nullptr, nullptr, w3, v2, nullptr, nullptr, nullptr, 4, nu, stream);
+        case 5: return fk_run_pass(pl, sup, nullptr, ys[mask], w3, v2, nullptr, nullptr, nullptr, 5, nu, stream);
+        default: return fail(D4W_ERR_ARG, "d4w_fk_bank_apply_pass: pass must be 1..5");
+    }
+}
+
+extern "C" int d4w_fk_bank_apply(d4w_fk_plan* pl, d4w_fk_bank* b, const float* x, float* const* ys, void* ws, int taper,
+                                 void* stream) {
+    int rc = d4w_fk_bank_apply_pass(pl, b, x, ys, ws, taper, 1, 0, stream);
+    if (rc == D4W_OK) rc = d4w_fk_bank_apply_pass(pl, b, x, ys, ws, taper, 2, 0, stream);
+    for (int i = 0; rc == D4W_OK && b && i < (int)b->masks.size(); ++i)
+        for (int pass = 3; rc == D4W_OK && pass <= 5; ++pass) rc = d4w_fk_bank_apply_pass(pl, b, x, ys, ws, taper, pass, i, stream);
+    return rc;
 }

@@ -133,6 +133,14 @@ __host__ __device__ inline void body_mask_build(const MaskParams& mp, float* tab
     tab[idx] = (float)(mask_folded(mp, act_k[slot], f) * scale);
 }
 
+// mask bank table: row u of the bank's union support takes row src_row[u] of the mask's own table, or exact zeros
+// where the mask does not keep that wavenumber (src_row[u] < 0), so a pruned mask's dropped rows stay dropped
+__host__ __device__ inline void body_bank_gather(const float* __restrict__ src, float* __restrict__ dst,
+                                                 const int* __restrict__ src_row, int ns, size_t idx) {
+    const int r = src_row[idx / ns];
+    dst[idx] = r < 0 ? 0.f : src[(size_t)r * ns + idx % ns];
+}
+
 // ------------------------------------------------------------------ async copy helpers
 #ifdef __CUDACC__
 __device__ __forceinline__ void cp_async8(void* smem_dst, const void* gsrc) {
@@ -521,10 +529,11 @@ __host__ __device__ inline void body_row_split(float2* __restrict__ w, size_t ld
 // `tab` is indexed [slot*tab_slot_stride + kt1*T2 + p] in transform (digit-reversed) order;
 // tab_slot_stride = 0 shares one table between all rows (Hilbert weights, template spectra).
 // TabT = float2 (the chirp-z Hilbert rows' kernel spectrum): the table multiplies instead of scaling.
-template <typename TabT>
+// OOP (mask banks): read the tile from w, write the result to the same place in `dst` (same layout), w untouched.
+template <typename TabT, bool OOP = false>
 __host__ __device__ inline void body_row_mid(const RowParams& rp, float2* __restrict__ w, size_t ldw,
                                              const TabT* __restrict__ tab, size_t tab_slot_stride, int kt1, int slot,
-                                             int tid, int nthr, float2* smem) {
+                                             int tid, int nthr, float2* smem, float2* __restrict__ dst = nullptr) {
     const int n = rp.t2;
     float2* g = w + (size_t)slot * ldw + (size_t)kt1 * n;
     bool staged = false;
@@ -549,7 +558,12 @@ __host__ __device__ inline void body_row_mid(const RowParams& rp, float2* __rest
     }
     D4W_SYNC();
     fft_inverse_stages(smem, rp.pl, rp.tw, 1, n, tid, nthr, 0, rp.pl.nstages);
-    for (int i = tid; i < n; i += nthr) g[i] = smem[i];
+    if constexpr (OOP) {
+        float2* o = dst + (size_t)slot * ldw + (size_t)kt1 * n;
+        for (int i = tid; i < n; i += nthr) o[i] = smem[i];
+    } else {
+        for (int i = tid; i < n; i += nthr) g[i] = smem[i];
+    }
 }
 
 
@@ -557,9 +571,10 @@ __host__ __device__ inline void body_row_mid(const RowParams& rp, float2* __rest
 // Rows slotA = 2*pair, slotB = slotA + 1 (same kt1 tile) are interleaved on the way into shared memory
 // ({reA, reB, imA, imB} per sample), share every butterfly / twiddle, and each lane is multiplied by its
 // own row of the mask table.  An odd trailing row runs with lane B = 0.
+template <bool OOP = false>
 __host__ __device__ inline void body_row_mid_dual(const RowParams& rp, float2* __restrict__ w, size_t ldw,
                                                   const float* __restrict__ tab, size_t tab_slot_stride, int kt1, int pair,
-                                                  int nslots, int tid, int nthr, cpd* smem) {
+                                                  int nslots, int tid, int nthr, cpd* smem, float2* __restrict__ dst = nullptr) {
     const int n = rp.t2;
     const int sa = 2 * pair, sb = sa + 1;
     const bool has_b = sb < nslots;
@@ -584,10 +599,20 @@ __host__ __device__ inline void body_row_mid_dual(const RowParams& rp, float2* _
     }
     D4W_SYNC();
     fft_inverse_stages_dual(smem, rp.pl, rp.tw, 1, n, tid, nthr);
-    for (int i = tid; i < n; i += nthr) {
-        const cpd v = smem[i];
-        ga[i] = make_float2(f2x_lo(v.x), f2x_lo(v.y));
-        if (has_b) gb[i] = make_float2(f2x_hi(v.x), f2x_hi(v.y));
+    if constexpr (OOP) {
+        float2* oa = dst + (size_t)sa * ldw + (size_t)kt1 * n;
+        float2* ob = dst + (size_t)(has_b ? sb : sa) * ldw + (size_t)kt1 * n;
+        for (int i = tid; i < n; i += nthr) {
+            const cpd v = smem[i];
+            oa[i] = make_float2(f2x_lo(v.x), f2x_lo(v.y));
+            if (has_b) ob[i] = make_float2(f2x_hi(v.x), f2x_hi(v.y));
+        }
+    } else {
+        for (int i = tid; i < n; i += nthr) {
+            const cpd v = smem[i];
+            ga[i] = make_float2(f2x_lo(v.x), f2x_lo(v.y));
+            if (has_b) gb[i] = make_float2(f2x_hi(v.x), f2x_hi(v.y));
+        }
     }
 }
 
@@ -1040,10 +1065,10 @@ __host__ __device__ inline void row_last_masked(float2* __restrict__ s, const Ta
 __host__ __device__ inline bool row_radix_inreg(int r) {
     return r == 2 || r == 3 || r == 4 || r == 5 || r == 6 || r == 8 || r == 10 || r == 12 || r == 15 || r == 16 || r == 20 || r == 25;
 }
-template <typename TabT>
+template <typename TabT, bool OOP = false>
 __host__ __device__ inline void body_row_mid_fused(const RowParams& rp, float2* __restrict__ w, size_t ldw,
                                                    const TabT* __restrict__ tab, size_t tab_slot_stride, int kt1, int slot,
-                                                   int tid, int nthr, float2* smem) {
+                                                   int tid, int nthr, float2* smem, float2* __restrict__ dst = nullptr) {
     const int n = rp.t2, nst = rp.pl.nstages;
     float2* g = w + (size_t)slot * ldw + (size_t)kt1 * n;
     const TabT* m = tab + (size_t)slot * tab_slot_stride + (size_t)kt1 * n;
@@ -1058,9 +1083,16 @@ __host__ __device__ inline void body_row_mid_fused(const RowParams& rp, float2* 
 #undef D4W_CALL
     D4W_SYNC();
     fft_inverse_stages(smem, rp.pl, rp.tw, 1, n, tid, nthr, 1, nst - 1);
-#define D4W_CALL(R) row_first_inv<R>(g, smem, rp.tw, n, tid, nthr);
-    D4W_ROW_RADIX_SWITCH(r0, D4W_CALL)
+    if constexpr (OOP) {
+        float2* o = dst + (size_t)slot * ldw + (size_t)kt1 * n;
+#define D4W_CALL(R) row_first_inv<R>(o, smem, rp.tw, n, tid, nthr);
+        D4W_ROW_RADIX_SWITCH(r0, D4W_CALL)
 #undef D4W_CALL
+    } else {
+#define D4W_CALL(R) row_first_inv<R>(g, smem, rp.tw, n, tid, nthr);
+        D4W_ROW_RADIX_SWITCH(r0, D4W_CALL)
+#undef D4W_CALL
+    }
 }
 
 // ================================================================== __global__ wrappers

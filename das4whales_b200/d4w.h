@@ -109,6 +109,35 @@ int d4w_fk_apply_pass_ex(d4w_fk_plan* plan, d4w_fk_mask* mask, const float* dev_
                          void* dev_workspace, int taper, int pass, int slot_begin, int slot_count,
                          int t_offset, void* stream);
 
+/* ---- f-k mask bank: several masks over one plan and one forward transform (scripts/main_fkcomp.py:66-95
+ *      filters the same matrix with four masks, each through dsp.fk_filter_sparsefilt, :73-95) ----------- */
+typedef struct d4w_fk_bank d4w_fk_bank;
+/* The bank keeps the union U of the masks' kept wavenumber rows, each mask's support taken as it is now (after
+ * d4w_fk_mask_prune, if any).  Every mask must be of `plan`, built (d4w_fk_mask_build) before d4w_fk_bank_build,
+ * not pruned again, and must outlive the bank.  D4W_ERR_ARG: nmasks < 1, a null mask, a mask of another plan. */
+int d4w_fk_bank_create(d4w_fk_bank** out, d4w_fk_plan* plan, d4w_fk_mask* const* masks, int nmasks);
+int d4w_fk_bank_destroy(d4w_fk_bank* bank);
+/* |U|, the rows every mask of the bank is filtered on */
+int d4w_fk_bank_rows(const d4w_fk_bank* bank);
+/* bytes of device memory for the bank's tables: nmasks x |U| x ns float32 */
+size_t d4w_fk_bank_table_bytes(const d4w_fk_bank* bank);
+/* fill the caller's table (kept by reference until the bank is destroyed): mask i's own transform-order table on the
+ * slots of its kept rows and exact zeros on the other slots of U, so a pruned mask's dropped rows stay dropped */
+int d4w_fk_bank_build(d4w_fk_bank* bank, float* dev_table, void* stream);
+/* bytes of workspace for d4w_fk_bank_apply: two blocks of |U| kept rows (the forward transform and one mask's
+ * filtered rows), plus the level-A/B intermediate of a two-level plan */
+size_t d4w_fk_bank_workspace_bytes(const d4w_fk_plan* plan, const d4w_fk_bank* bank);
+/* dev_ys[i] = d4w_fk_apply(plan, mask i, dev_x) for every mask, with one forward transform: P1 (optional taper, as
+ * d4w_fk_apply) and P2 once, then for each mask P3 out of place into the second block, P4 and P5 into dev_ys[i].
+ * dev_ys is a host array of nmasks device pointers.  One output may alias x; outputs may not overlap each other
+ * (D4W_ERR_ARG), nor may the bank be applied before d4w_fk_bank_build. */
+int d4w_fk_bank_apply(d4w_fk_plan* plan, d4w_fk_bank* bank, const float* dev_x, float* const* dev_ys,
+                      void* dev_workspace, int taper, void* stream);
+/* the passes separately (profiling): passes 1 and 2 serve every mask, passes 3..5 run mask `mask` (pass 5 writes
+ * dev_ys[mask]); 1, 2, then 3, 4, 5 for each mask in turn is d4w_fk_bank_apply */
+int d4w_fk_bank_apply_pass(d4w_fk_plan* plan, d4w_fk_bank* bank, const float* dev_x, float* const* dev_ys,
+                           void* dev_workspace, int taper, int pass, int mask, void* stream);
+
 /* ---- generic shared-memory FFT plan (matched-filter blocks, STFT frames) ----------------- */
 typedef struct d4w_fft_plan d4w_fft_plan;
 typedef struct d4w_row_plan d4w_row_plan;

@@ -253,6 +253,27 @@ def fk_filter_sparsefilt(trace, fk_filter_matrix, tapering=False):
     return fk_filter_filt(trace, fk_filter_matrix, tapering=tapering)
 
 
+def fk_filter_filts(trace, fk_filter_matrices, tapering=False):
+    """fk_filter_filt of one trace with several masks (what scripts/main_fkcomp.py:73-95 does with four
+    fk_filter_sparsefilt calls), through one forward transform (fk.FkFilterBank).  Each output equals
+    fk_filter_filt(trace, mask_i, tapering).  An ndarray goes up once and gives a list of float64 ndarrays; a CUDA
+    tensor gives a list of float32 tensors.  `tapering=True` tapers the caller's array once, in place."""
+    if _is_tensor(trace):
+        x = _to_device(trace)
+        bank = _fk.FkFilterBank(fk_filter_matrices, shape=tuple(x.shape), device=x.device.index)
+        ys = bank(x, tapering=tapering)
+        if tapering:
+            _taper_edges_inplace(trace)
+        return ys
+    arr = np.asarray(trace)
+    x = _to_device(arr)
+    bank = _fk.FkFilterBank(fk_filter_matrices, shape=tuple(x.shape))
+    ys = bank(x, outs=[x] + [_fk._torch().empty_like(x) for _ in range(len(bank) - 1)], tapering=tapering)
+    if tapering and isinstance(trace, np.ndarray) and trace.flags.writeable and np.issubdtype(trace.dtype, np.floating):
+        _taper_edges_inplace(trace)
+    return [_to_host64(y) for y in ys]
+
+
 # ------------------------------------------------------------------------------ IIR
 def butterworth_filter(filterspec, fs):
     """SOS Butterworth design (reference: dsp.py:789-827) -- design only, host side."""

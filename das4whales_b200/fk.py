@@ -326,8 +326,97 @@ class FkFilter:
 
     def traffic_bytes(self):
         """Actual HBM bytes each pass must move (for the per-kernel bandwidth report)."""
-        nx, ns, r = self.plan.nx, self.plan.ns, self.rows_kept
-        real, spec = nx * ns * 4, r * ns * 8
-        split = 2 * spec if self.plan.t1 > 1 else 0
-        return {"p1_col_fwd": real + spec, "p2_row_split": split, "p3_row_mid": 2 * spec + r * ns * 4,
-                "p4_row_unsplit": split, "p5_col_inv": spec + real}
+        return _traffic_bytes(self.plan, self.rows_kept)
+
+
+def _traffic_bytes(plan, r, nmasks=1):
+    nx, ns = plan.nx, plan.ns
+    real, spec = nx * ns * 4, r * ns * 8
+    split = 2 * spec if plan.t1 > 1 else 0
+    return {"p1_col_fwd": real + spec, "p2_row_split": split, "p3_row_mid": nmasks * (2 * spec + r * ns * 4),
+            "p4_row_unsplit": nmasks * split, "p5_col_inv": nmasks * (spec + real)}
+
+
+def _destroy_bank(lib, ptr, dms):
+    """Destroy a d4w_fk_bank; `dms` holds its masks (and their tables) until the bank is gone."""
+    lib.d4w_fk_bank_destroy(ptr)
+
+
+class FkFilterBank:
+    """Several f-k masks over one matrix shape, sharing one forward transform (d4w_fk_bank).
+
+    >>> bank = FkFilterBank([m1, m2, m3], device=0)   # masks: anything FkFilter accepts
+    >>> y1, y2, y3 = bank(x_cuda)                       # each equal to FkFilter(m_i)(x_cuda)
+
+    The rows filtered are the union of the masks' kept wavenumber rows (`rows_kept`); a mask is exactly zero on the
+    rows it does not keep, so each output equals the single-mask filter's.  `eps` / `mask.prune_eps` prune each mask
+    as FkFilter does."""
+
+    def __init__(self, masks, shape=None, device=None, eps=0.0):
+        torch = _torch()
+        masks = list(masks)
+        if not masks:
+            raise ValueError("FkFilterBank needs at least one mask")
+        self.device = torch.cuda.current_device() if device is None else int(device)
+        shape = tuple(shape) if shape is not None else tuple(masks[0].shape)
+        self.plan = get_plan(shape[0], shape[1], self.device)
+        L = _lib.lib()
+        out = _lib.ffi.new("d4w_fk_bank**")
+        with torch.cuda.device(self.device):
+            self.dms = [device_mask_for(m, self.plan, eps) for m in masks]
+            arr = _lib.ffi.new("d4w_fk_mask*[]", [dm.ptr for dm in self.dms])
+            _lib.check(L.d4w_fk_bank_create(out, self.plan.ptr, arr, len(self.dms)), "fk bank")
+            self.ptr = out[0]
+            weakref.finalize(self, _destroy_bank, L, self.ptr, self.dms)
+            self.rows_kept = L.d4w_fk_bank_rows(self.ptr)
+            nbytes = L.d4w_fk_bank_table_bytes(self.ptr)
+            self.table = torch.empty(int(nbytes) // 4, dtype=torch.float32, device=f"cuda:{self.device}")
+            _lib.check(L.d4w_fk_bank_build(self.ptr, _lib.ptr(self.table, "float*"), _lib.stream_ptr()), "fk bank build")
+            self.workspace_bytes = L.d4w_fk_bank_workspace_bytes(self.plan.ptr, self.ptr)
+        self.masks = masks
+
+    def __len__(self):
+        return len(self.dms)
+
+    def _ws(self):
+        return self.plan.get_workspace(self.workspace_bytes)
+
+    def _outs(self, x, outs):
+        torch = _torch()
+        if x.dtype != torch.float32 or not x.is_cuda or not x.is_contiguous():
+            raise ValueError("FkFilterBank expects a contiguous float32 CUDA tensor")
+        if tuple(x.shape) != (self.plan.nx, self.plan.ns):
+            raise ValueError(f"FkFilterBank built for {(self.plan.nx, self.plan.ns)}, got {tuple(x.shape)}")
+        if outs is None:
+            outs = [torch.empty_like(x) for _ in self.dms]
+        outs = list(outs)
+        if len(outs) != len(self.dms):
+            raise ValueError(f"FkFilterBank has {len(self.dms)} masks, got {len(outs)} outputs")
+        for o in outs:
+            if o.dtype != torch.float32 or not o.is_cuda or not o.is_contiguous() or tuple(o.shape) != tuple(x.shape) \
+                    or o.device != x.device:
+                raise ValueError("FkFilterBank outputs must be contiguous float32 CUDA tensors of the input's shape")
+        return outs, _lib.ffi.new("float*[]", [_lib.ptr(o, "float*") for o in outs])
+
+    def __call__(self, x, outs=None, tapering=False):
+        """Filter x with every mask; returns the list of outputs.  One of `outs` may be x itself; no two may overlap."""
+        outs, ys = self._outs(x, outs)
+        L = _lib.lib()
+        with _torch().cuda.device(self.device):
+            _lib.check(L.d4w_fk_bank_apply(self.plan.ptr, self.ptr, _lib.ptr(x, "float*"), ys, _lib.ptr(self._ws()),
+                                           int(bool(tapering)), _lib.stream_ptr()), "fk bank")
+        return outs
+
+    def run_pass(self, i, x, outs, tapering=False, mask=0):
+        """Launch pass i (1..5) alone -- profiling / per-kernel timing.  Passes 1 and 2 serve every mask; passes 3..5
+        run mask `mask`."""
+        outs, ys = self._outs(x, outs)
+        L = _lib.lib()
+        with _torch().cuda.device(self.device):
+            _lib.check(L.d4w_fk_bank_apply_pass(self.plan.ptr, self.ptr, _lib.ptr(x, "float*"), ys, _lib.ptr(self._ws()),
+                                                int(bool(tapering)), int(i), int(mask), _lib.stream_ptr()),
+                       f"fk bank pass {i}")
+
+    def traffic_bytes(self):
+        """HBM bytes each pass must move for the whole bank (passes 3..5 summed over the masks)."""
+        return _traffic_bytes(self.plan, self.rows_kept, len(self.dms))

@@ -24,6 +24,9 @@ find_peaks with an absolute prominence on the raw correlograms (detect.pick_time
 (envelope median and mean, std, SNR_1d, and the power and mean envelope of a noise window) from two envelope-statistics
 passes (rows.env_stats); it yields [nx]-long float64 vectors instead of picks.
 
+`FkCompPipeline` is scripts/main_fkcomp.py:56-122: strain and band-pass as above, then the script's four f-k masks through one
+forward transform (fk.FkFilterBank), the argmax and cross-section of the inf_cos output and the envelope SNR of every output.
+
 Only the raw counts go up (pinned int32, 4 bytes per sample) and only the picks come down; every intermediate matrix
 stays in HBM.  `stream(files)` overlaps the H2D copy of file i+1 with the processing of file i.
 """
@@ -41,6 +44,8 @@ class _FilePipeline:
     threshold-and-pick tail, and the double-buffered upload of `stream`.  Subclasses implement process_device(raw) on top
     of _filtered and _pick (or their own picking tail)."""
 
+    _hybrid_ninf_front_end = True      # False: the subclass filters with masks of its own, and no FkFilter is built here
+
     def __init__(self, nx, ns, selected_channels, dx, fs, scale_factor, device, fmin, fmax, mask_speeds, thres_frac,
                  prune_eps, bandpass):
         import scipy.signal as sp
@@ -51,18 +56,24 @@ class _FilePipeline:
         self.scale_factor = float(scale_factor)
         self.thres_frac = None if thres_frac is None else float(thres_frac)      # None: the subclass picks by its own rule
         self.bandpass = bool(bandpass)
-        with torch.cuda.device(self.device):
-            self.mask = _dsp.hybrid_ninf_filter_design((nx, ns), selected_channels, dx, fs, *mask_speeds, fmin=fmin, fmax=fmax)
-            self.fk = _fk.FkFilter(self.mask, device=self.device, eps=prune_eps)
+        if self._hybrid_ninf_front_end:
+            with torch.cuda.device(self.device):
+                self.mask = _dsp.hybrid_ninf_filter_design((nx, ns), selected_channels, dx, fs, *mask_speeds, fmin=fmin,
+                                                           fmax=fmax)
+                self.fk = _fk.FkFilter(self.mask, device=self.device, eps=prune_eps)
         self.sos = sp.butter(8, [fmin / (fs / 2), fmax / (fs / 2)], "bp", output="sos")          # dsp.bp_filt (dsp.py:878)
         self._raw = [None, None]
         self._h2d = None
 
     # ---- device side -------------------------------------------------------------------------------------------------
-    def _filtered(self, raw):
+    def _bandpassed(self, raw):
         x = _rows.raw2strain(raw, self.scale_factor)
         if self.bandpass:
             x = _rows.sosfiltfilt(self.sos, x, padlen=3 * 17)
+        return x
+
+    def _filtered(self, raw):
+        x = self._bandpassed(raw)
         return self.fk(x, out=x)
 
     def _maxv(self, corr):
@@ -274,6 +285,65 @@ class NoiseProfilePipeline(_FilePipeline):
         return {k: v.cpu().numpy() for k, v in res.items()}
 
 
+FKCOMP_MASKS = ("nf_cos", "nf_gs", "inf_cos", "inf_gs")       # scripts/main_fkcomp.py:73-95, in the script's order
+
+
+class FkCompPipeline(_FilePipeline):
+    """scripts/main_fkcomp.py:56-122 on the device; the script's values are the defaults.  The band-passed strain is
+    filtered with the script's four masks through one forward transform (fk.FkFilterBank):
+
+        nf_cos   dsp.hybrid_ninf_filter_design      (:73-76)
+        nf_gs    dsp.hybrid_ninf_gs_filter_design   (:79-82)
+        inf_cos  dsp.hybrid_filter_design           (:86-89, cs_min and cp_min only)
+        inf_gs   dsp.hybrid_gs_filter_design        (:92-95, cs_min and cp_min only)
+
+    then the argmax of inf_cos, its cross-section at that time (:104-106) and snr_tr_array(env=True) of each output
+    (:113-122).  The masks are designed once, here."""
+
+    _hybrid_ninf_front_end = False
+
+    def __init__(self, nx, ns, selected_channels, dx, fs, scale_factor, device=None, fmin=14., fmax=30.,
+                 mask_speeds=(1350., 1450., 3300., 3450.), prune_eps=0.0, bandpass=True):
+        super().__init__(nx, ns, selected_channels, dx, fs, scale_factor, device, fmin, fmax, mask_speeds, None,
+                         prune_eps, bandpass)
+        cs_min, cp_min, cp_max, cs_max = (float(c) for c in mask_speeds)
+        shape, sel = (int(nx), int(ns)), list(selected_channels)
+        finite = dict(cs_min=cs_min, cp_min=cp_min, cp_max=cp_max, cs_max=cs_max, fmin=fmin, fmax=fmax)
+        infinite = dict(cs_min=cs_min, cp_min=cp_min, fmin=fmin, fmax=fmax)
+        with self.torch.cuda.device(self.device):
+            masks = [_dsp.hybrid_ninf_filter_design(shape, sel, dx, fs, **finite),
+                     _dsp.hybrid_ninf_gs_filter_design(shape, sel, dx, fs, **finite),
+                     _dsp.hybrid_filter_design(shape, sel, dx, fs, **infinite),
+                     _dsp.hybrid_gs_filter_design(shape, sel, dx, fs, **infinite)]
+            self.masks = dict(zip(FKCOMP_MASKS, masks))
+            self.bank = _fk.FkFilterBank(masks, device=self.device, eps=prune_eps)
+
+    def process_device(self, raw, with_traces=False):
+        """raw: int32 (or float32) CUDA tensor [nx, ns] of interrogator counts.  Returns a dict of DEVICE results:
+        snr = {name: float32 [nx, ns]} (snr_tr_array(env=True) of each output, :113-122), argmax = (xi_m, tj_m) of the
+        inf_cos output (the first maximum in C order, as np.argmax, :104), section = inf_cos[:, tj_m] (:106) and, with
+        with_traces, traces = {name: float32 [nx, ns]} (the four filtered matrices)."""
+        torch = self.torch
+        with torch.cuda.device(self.device):
+            x = self._bandpassed(raw)
+            ys = self.bank(x, outs=[x] + [torch.empty_like(x) for _ in FKCOMP_MASKS[1:]])
+            traces = dict(zip(FKCOMP_MASKS, ys))
+            inf = traces["inf_cos"]
+            xi_m, tj_m = divmod(int(torch.argmax(inf).item()), self.ns)
+            out = {"snr": {k: _rows.snr(y, env=True) for k, y in traces.items()}, "argmax": (xi_m, tj_m),
+                   "section": inf[:, tj_m].clone()}
+            if with_traces:
+                out["traces"] = traces
+            return out
+
+    def _to_host(self, res):
+        out = {"snr": {k: v.to(self.torch.float64).cpu().numpy() for k, v in res["snr"].items()},
+               "argmax": res["argmax"], "section": res["section"].to(self.torch.float64).cpu().numpy()}
+        if "traces" in res:
+            out["traces"] = {k: _dsp._to_host64(v) for k, v in res["traces"].items()}
+        return out
+
+
 def process_file(raw, metadata, selected_channels, **kw):
     """Convenience wrapper: raw [nx, ns] counts + the reference's metadata dict (data_handle.get_acquisition_parameters:
     fs, dx, scale_factor) -> picks of the HF and LF fin-whale notes."""
@@ -295,6 +365,15 @@ def process_file_spectro(raw, metadata, selected_channels, **kw):
     scale_factor) -> frame-index picks of the HF and LF notes of scripts/main_spectrodetect.py."""
     nx, ns = raw.shape
     pipe = SpectroDetectPipeline(nx, ns, selected_channels, metadata["dx"], metadata["fs"], metadata["scale_factor"], **kw)
+    return pipe.process_file(raw)
+
+
+def process_file_fkcomp(raw, metadata, selected_channels, **kw):
+    """Convenience wrapper of FkCompPipeline: raw [nx, ns] counts + the reference's metadata dict (fs, dx,
+    scale_factor) -> the f-k mask comparison of scripts/main_fkcomp.py (SNR matrices, argmax and cross-section of the
+    inf_cos output, float64 on the host)."""
+    nx, ns = raw.shape
+    pipe = FkCompPipeline(nx, ns, selected_channels, metadata["dx"], metadata["fs"], metadata["scale_factor"], **kw)
     return pipe.process_file(raw)
 
 
