@@ -222,6 +222,25 @@ int d4w_stft_slide_supported(int nfft, int hop, int nbins);
 int d4w_stft_slide(d4w_fft_plan* plan, const float* x, float* out, int nx, int ns, int hop, int bin_lo, int bin_hi,
                    void* stream);
 
+/* ---- Welch power spectral density of every chunk of every row: tools.spec / tools.__spec_chunk
+ *      (/root/reference/src/das4whales/tools.py:212-236), scipy.signal.welch(chunk, fs, window, nperseg, noverlap, nfft,
+ *      detrend, return_onesided=True, scaling, average) per chunk.  Row r, chunk c is the `chunk` samples at
+ *      dev_x + r * ns + c * chunk, c < ns / chunk (chunk = ns: the whole row).  Segment s of a chunk covers samples
+ *      [s * step, s * step + nperseg), nseg = (chunk - nperseg) / step + 1 (step = nperseg - noverlap; a trailing partial
+ *      segment is dropped, no padding, no centring).  detrend != 0 subtracts each segment's mean; the segment is multiplied by
+ *      dev_window[nperseg] and zero-padded to nfft = the plan's length.  The periodogram |X_k|^2 * scale (scale = 1 / (fs * sum
+ *      w^2) for a density, 1 / (sum w)^2 for a spectrum) is doubled at every bin but DC and, for even nfft, Nyquist (SciPy's
+ *      one-sided rule), then averaged over the segments: average 0 = mean, 1 = np.median / _median_bias(nseg).
+ *      dev_out: float32 [nrows][ns / chunk][nfft / 2 + 1].  Every nfft the plan accepts whose one complex frame (plus the bin
+ *      sums) fits shared memory: D4W_ERR_UNSUPPORTED names the limit.  D4W_ERR_ARG: nrows < 1, chunk outside [1, ns],
+ *      nperseg outside [1, chunk], step < 1, nfft < nperseg.
+ *      dev_workspace: d4w_welch_workspace_bytes bytes (0 unless a median over more segments than fit shared memory, which
+ *      writes every periodogram bin-major for d4w_row_median: nrows x nchunks x nbins x nseg floats). */
+size_t d4w_welch_workspace_bytes(const d4w_fft_plan* plan, int nrows, int ns, int chunk, int nperseg, int step, int average);
+int d4w_welch(d4w_fft_plan* plan, const float* dev_x, int nrows, int ns, int chunk, int nperseg, int step,
+              const float* dev_window, int detrend, double scale, int average, float* dev_out, void* dev_workspace,
+              void* stream);
+
 /* ---- spectrogram-correlation detector: detect.xcorr2d / compute_cross_correlogram_spectrocorr
  *      (detect.py:579-602, :650-708).  Per-row median / maximum of a float32 matrix [nrows][n]
  *      (entries must be >= 0 for the median), and

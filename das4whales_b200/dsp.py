@@ -5,6 +5,9 @@ on hand-written sm_90a CUDA kernels (libd4w.so) instead of NumPy/SciPy.
 Accepted data: `numpy.ndarray` (any float dtype; the result is a new float64 ndarray, as the
 reference returns) or a CUDA `torch.Tensor` (float32; the result stays on the device).
 """
+import warnings
+from collections import namedtuple
+
 import numpy as np
 import scipy.signal as sp
 
@@ -345,6 +348,118 @@ def snr_tr_array(trace, env=False):
     xd = _to_device(trace)
     y = _rows.snr(xd, env=bool(env))
     return y if _is_tensor(trace) else _to_host64(y)
+
+
+# ------------------------------------------------------------------------------ Welch power spectral density
+WelchLayout = namedtuple("WelchLayout", "nperseg noverlap step nfft chunk nchunks nseg nbins median_bias")
+
+
+def _largest_prime_factor(n):
+    p, big = 2, 1
+    while p * p <= n:
+        while n % p == 0:
+            big, n = p, n // p
+        p += 1
+    return max(big, n)
+
+
+def welch_layout(ns, nperseg, noverlap=None, nfft=None, chunk=None):
+    """Segments and bins of scipy.signal.welch over whole chunks of ns-sample rows, pure Python (d4w_welch's geometry).
+    noverlap=None is nperseg // 2, nfft=None is nperseg, chunk=None is the whole row.  Segment s of a chunk covers samples
+    [s * step, s * step + nperseg), step = nperseg - noverlap, nseg = (chunk - nperseg) // step + 1 (no padding; a
+    trailing partial segment is dropped).  median_bias = SciPy's _median_bias(nseg).  ValueError for inconsistent sizes
+    and for an nfft with a prime factor above 61, which the shared-memory FFT does not take."""
+    ns, nperseg = int(ns), int(nperseg)
+    chunk = ns if chunk is None else int(chunk)
+    if ns < 1:
+        raise ValueError("welch: empty input")
+    if not 1 <= chunk <= ns:
+        raise ValueError(f"chunk = {chunk} must be in [1, {ns}]")
+    if nperseg < 1:
+        raise ValueError(f"nperseg = {nperseg} is not a positive integer")
+    if nperseg > chunk:
+        raise ValueError(f"nperseg = {nperseg} is longer than the chunk of {chunk} samples")
+    nfft = nperseg if nfft is None else int(nfft)
+    if nfft < nperseg:
+        raise ValueError(f"nfft = {nfft} must be greater than or equal to nperseg = {nperseg}")
+    noverlap = nperseg // 2 if noverlap is None else int(noverlap)
+    if noverlap >= nperseg:
+        raise ValueError(f"noverlap = {noverlap} must be less than nperseg = {nperseg}")
+    if nfft < 2 or _largest_prime_factor(nfft) > 61:
+        raise ValueError(f"nfft = {nfft}: the shared-memory FFT takes lengths >= 2 whose prime factors are all <= 61")
+    step = nperseg - noverlap
+    nseg = (chunk - nperseg) // step + 1
+    ii = 2.0 * np.arange(1.0, (nseg - 1) // 2 + 1)
+    bias = float(1.0 + np.sum(1.0 / (ii + 1) - 1.0 / ii))
+    return WelchLayout(nperseg, noverlap, step, nfft, chunk, ns // chunk, nseg, nfft // 2 + 1, bias)
+
+
+def welch_window(window, nperseg, ns):
+    """(window values float64 [nperseg], nperseg) by scipy.signal.welch's rules: a string or tuple is
+    scipy.signal.get_window(window, nperseg) with nperseg=None meaning 256, cut to ns with SciPy's warning when longer than
+    the input; an array gives nperseg = its length and must match nperseg when both are given."""
+    if isinstance(window, (str, tuple)):
+        nperseg = 256 if nperseg is None else int(nperseg)
+        if nperseg < 1:
+            raise ValueError(f"nperseg = {nperseg} is not a positive integer")
+        if ns < nperseg:
+            warnings.warn(f"nperseg={nperseg} is greater than signal length max(len(x), len(y)) = {ns}, using nperseg = {ns}",
+                          stacklevel=3)
+            nperseg = ns
+        return np.asarray(sp.get_window(window, nperseg), dtype=np.float64), nperseg
+    win = np.asarray(window)
+    if win.ndim != 1 or np.iscomplexobj(win):
+        raise ValueError("an array window must be real and 1-D")
+    nperseg = len(win) if nperseg is None else int(nperseg)
+    if nperseg != len(win):
+        raise ValueError(f"nperseg={nperseg} does not equal len(win)={len(win)}")
+    if nperseg > ns:
+        raise ValueError(f"window of {nperseg} samples is longer than the input of {ns}")
+    return win.astype(np.float64), nperseg
+
+
+def welch_scale(win, fs, scaling):
+    """SciPy's periodogram scale: 1 / (fs sum w^2) for 'density', 1 / (sum w)^2 for 'spectrum'"""
+    win = np.asarray(win, dtype=np.float64)
+    if scaling == "density":
+        return 1.0 / (fs * float(np.sum(win * win)))
+    if scaling == "spectrum":
+        return 1.0 / float(np.sum(win)) ** 2
+    raise ValueError(f"Parameter scaling={scaling!r} not in {{'spectrum': 'magnitude', 'density': 'psd'}}!")
+
+
+def welch(x, fs=1.0, window="hann_periodic", nperseg=None, noverlap=None, nfft=None, detrend="constant",
+          return_onesided=True, scaling="density", axis=-1, average="mean"):
+    """scipy.signal.welch (SciPy 1.18 defaults) of 1-D or 2-D real input along the last axis, every row in one d4w_welch
+    call.  Returns (f, Pxx): f = rfftfreq(nfft, 1 / fs) as a float64 ndarray; Pxx [nbins] or [nrows, nbins], a float64
+    ndarray for an ndarray in and a float32 CUDA tensor for a tensor in.  ValueError, with no fall-back to SciPy, for what
+    the kernel does not compute: detrend other than 'constant' or False, return_onesided=False, another axis, complex input."""
+    tensor = _is_tensor(x)
+    a = x if tensor else np.asarray(x)
+    if a.ndim not in (1, 2):
+        raise ValueError(f"welch takes 1-D or 2-D input, not {a.ndim}-D")
+    if int(axis) not in (-1, a.ndim - 1):
+        raise ValueError("welch computes along the last axis only (axis=-1)")
+    if (a.is_complex() if tensor else np.iscomplexobj(a)):
+        raise ValueError("welch takes real input only")
+    if not return_onesided:
+        raise ValueError("welch computes one-sided spectra only (return_onesided=True)")
+    if detrend is not False and detrend != "constant":
+        raise ValueError(f"detrend={detrend!r}: only 'constant' and False are computed")
+    if average not in ("mean", "median"):
+        raise ValueError(f"Parameter average={average!r} must be 'median' or 'mean'!")
+    ns = int(a.shape[-1])
+    win, nperseg = welch_window(window, nperseg, ns)
+    lay = welch_layout(ns, nperseg, noverlap, nfft)
+    scale = welch_scale(win, fs, scaling)
+    xd = _to_device(a)
+    if xd.ndim == 1:
+        xd = xd.reshape(1, -1)
+    p = _rows.welch(xd, lay.nperseg, lay.step, lay.nfft, win, detrend == "constant", scale, average)[:, 0, :]
+    f = np.fft.rfftfreq(lay.nfft, 1 / fs)
+    if a.ndim == 1:
+        p = p[0]
+    return f, (p if tensor else _to_host64(p))
 
 
 # ------------------------------------------------------------------------------ cable noise profile

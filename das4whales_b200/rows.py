@@ -397,6 +397,46 @@ def _stft_frames(x, nfft, hop, bin_lo, bin_hi):
     return out
 
 
+# ------------------------------------------------------------------------------ Welch power spectral density
+_WELCH_WS_ROWS_BYTES = 1 << 30      # rows per call are capped so that the median's periodogram workspace stays <= 1 GiB
+
+
+def welch(x, nperseg, step, nfft, window, detrend, scale, average, chunk=None):
+    """Welch PSD of every whole chunk of every row (d4w_welch): x contiguous float32 CUDA [nrows, ns]; segments of nperseg
+    samples every `step`, `window` (nperseg values, host), detrend = True for SciPy's 'constant', zero-padded to nfft,
+    `scale` = SciPy's 1 / (fs sum w^2) or 1 / (sum w)^2, average 'mean' or 'median'; chunk=None is the whole row.
+    Returns float32 CUDA [nrows, ns // chunk, nfft // 2 + 1]."""
+    torch = _torch()
+    dev = _check_input(x)
+    nx, ns = x.shape
+    chunk = ns if chunk is None else int(chunk)
+    if average not in ("mean", "median"):
+        raise ValueError(f"average must be 'mean' or 'median', not {average!r}")
+    med = 1 if average == "median" else 0
+    plan = fft_plan(int(nfft), dev)
+    win = np.ascontiguousarray(window, dtype=np.float32)
+    if win.shape != (int(nperseg),):
+        raise ValueError(f"window of shape {win.shape} for segments of {nperseg} samples")
+    wd = torch.from_numpy(win).to(x.device)          # nperseg floats per call: nothing cached per window
+    nchunks = ns // chunk if 1 <= chunk <= ns else 0
+    out = torch.empty((nx, nchunks, int(nfft) // 2 + 1), dtype=torch.float32, device=x.device)
+    L = _lib.lib()
+    args = (ns, chunk, int(nperseg), int(step), med)
+    per_row = int(L.d4w_welch_workspace_bytes(plan.ptr, 1, *args))
+    max_rows = nx if per_row == 0 else max(1, min(nx, _WELCH_WS_ROWS_BYTES // per_row))
+    with torch.cuda.device(dev):
+        ws = torch.empty(max(1, per_row * max_rows), dtype=torch.uint8, device=x.device)
+        for r0 in range(0, nx, max_rows):
+            r1 = min(nx, r0 + max_rows)
+            rc = L.d4w_welch(plan.ptr, _lib.ptr(x[r0:r1], "float*"), r1 - r0, ns, chunk, int(nperseg), int(step),
+                             _lib.ptr(wd, "float*"), 1 if detrend else 0, float(scale), med, _lib.ptr(out[r0:r1], "float*"),
+                             _lib.ptr(ws), _lib.stream_ptr())
+            if rc == 2:             # D4W_ERR_UNSUPPORTED: the nfft limit, named in the message
+                raise ValueError("welch: " + _lib.ffi.string(L.d4w_last_error()).decode(errors="replace"))
+            _lib.check(rc, "welch")
+    return out
+
+
 # ------------------------------------------------------------------------------ spectrogram correlation
 def row_max(x2d):
     """max over the last axis of a [rows, n] float32 CUDA tensor"""
