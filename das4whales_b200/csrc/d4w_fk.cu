@@ -173,7 +173,6 @@ extern "C" int d4w_fk_plan_create(d4w_fk_plan** out, int nx, int ns, int device)
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_col_fwd<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_col_inv<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_row_mid, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_row_mid_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_row_mid_dual, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap);
     if (e != cudaSuccess) {
         std::string msg = std::string("d4w_fk_plan_create: ") + cudaGetErrorString(e);
@@ -617,9 +616,9 @@ static int fk_run_pass(const d4w_fk_plan* pl, const d4w_fk_mask* m, const float*
             if (w3) return launch_row_mid_oop(false, pl->hostplan.row_fused, grid, pl->row_threads, pl->row_smem, pl->row, w, ldw,
                                               tab, (size_t)pl->ns, slot_count, w3, pl->device, stream);
             if (pl->hostplan.row_fused)
-                k_row_mid_fused<<<grid, pl->row_threads, pl->row_smem, stream>>>(pl->row, w, ldw, tab, (size_t)pl->ns);
-            else
-                k_row_mid<<<grid, pl->row_threads, pl->row_smem, stream>>>(pl->row, w, ldw, tab, (size_t)pl->ns);
+                return launch_row_mid_fused(grid, pl->row_threads, pl->row_smem, pl->row, w, ldw, tab, (size_t)pl->ns, nullptr,
+                                            pl->device, stream);
+            k_row_mid<<<grid, pl->row_threads, pl->row_smem, stream>>>(pl->row, w, ldw, tab, (size_t)pl->ns);
             D4W_CHECK_LAUNCH("k_row_mid");
             return D4W_OK;
         }

@@ -1,8 +1,8 @@
 // d4w_fk_bank.cu -- device side of the f-k mask bank (d4w_fk.cu: d4w_fk_bank_*): the out-of-place middle pass
 // (W -> W', one mask table per launch) and the gather of each mask's table onto the bank's union support.
 // The kernels live in a translation unit of their own so that every kernel of d4w_fk.o and d4w_rows.o compiles to the
-// same code as without them (ptxas allocates the spilling k_row_mid_fused differently when its non-inlined helpers
-// gain a second caller in the same module).  The bodies are fk_kernels.cuh's, shared with the host emulator.
+// same code as without them (ptxas allocates kernels differently when the non-inlined FFT stage helpers gain callers
+// in the same module).  The bodies are fk_kernels.cuh's, shared with the host emulator.
 #include "d4w_common.hpp"
 #include "fk_kernels.cuh"
 
@@ -12,12 +12,6 @@ static __global__ void __launch_bounds__(256, 2)
 k_row_mid_oop(RowParams rp, float2* __restrict__ w, size_t ldw, const float* __restrict__ tab, size_t tab_slot_stride,
               float2* __restrict__ dst) {
     body_row_mid<float, true>(rp, w, ldw, tab, tab_slot_stride, blockIdx.x, blockIdx.y, threadIdx.x, blockDim.x, d4w_dyn_smem, dst);
-}
-
-static __global__ void __launch_bounds__(256, 2)
-k_row_mid_fused_oop(RowParams rp, float2* __restrict__ w, size_t ldw, const float* __restrict__ tab, size_t tab_slot_stride,
-                    float2* __restrict__ dst) {
-    body_row_mid_fused<float, true>(rp, w, ldw, tab, tab_slot_stride, blockIdx.x, blockIdx.y, threadIdx.x, blockDim.x, d4w_dyn_smem, dst);
 }
 
 static __global__ void __launch_bounds__(128, 2)     // as k_row_mid_dual: radix-25 dual butterflies need ~190 registers
@@ -33,7 +27,7 @@ static __global__ void k_bank_gather(const float* src, float* dst, const int* sr
 }
 
 // P3 of a bank: same grid, block and shared memory as the in-place launch of d4w_fk.cu; dual: k_row_mid_dual_oop with
-// `nslots` rows, fused: k_row_mid_fused_oop, otherwise k_row_mid_oop
+// `nslots` rows, fused: k_row_mid_fused writing to dst, otherwise k_row_mid_oop
 int launch_row_mid_oop(bool dual, bool fused, dim3 grid, int threads, size_t smem, const RowParams& rp, float2* w, size_t ldw,
                        const float* tab, size_t tab_slot_stride, int nslots, float2* dst, int device, cudaStream_t stream) {
     static bool attr_done_dev[64] = {};      // opt in to the device's shared memory once per device, as plan creation does
@@ -41,12 +35,11 @@ int launch_row_mid_oop(bool dual, bool fused, dim3 grid, int threads, size_t sme
         int cap = 0;
         D4W_CUDA_TRY(cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
         D4W_CUDA_TRY(cudaFuncSetAttribute(k_row_mid_oop, cudaFuncAttributeMaxDynamicSharedMemorySize, cap));
-        D4W_CUDA_TRY(cudaFuncSetAttribute(k_row_mid_fused_oop, cudaFuncAttributeMaxDynamicSharedMemorySize, cap));
         D4W_CUDA_TRY(cudaFuncSetAttribute(k_row_mid_dual_oop, cudaFuncAttributeMaxDynamicSharedMemorySize, cap));
         attr_done_dev[device & 63] = true;
     }
+    if (fused) return launch_row_mid_fused(grid, threads, smem, rp, w, ldw, tab, tab_slot_stride, dst, device, stream);
     if (dual) k_row_mid_dual_oop<<<grid, threads, smem, stream>>>(rp, w, ldw, tab, tab_slot_stride, nslots, dst);
-    else if (fused) k_row_mid_fused_oop<<<grid, threads, smem, stream>>>(rp, w, ldw, tab, tab_slot_stride, dst);
     else k_row_mid_oop<<<grid, threads, smem, stream>>>(rp, w, ldw, tab, tab_slot_stride, dst);
     D4W_CHECK_LAUNCH("k_row_mid_oop");
     return D4W_OK;

@@ -143,7 +143,6 @@ static int row_plan_create_czt(d4w_row_plan** out, int ns, int device, const cud
     if (e == cudaSuccess) e = upload(&p->d_bhatc, bc);
     const int smax = (int)prop.sharedMemPerBlockOptin;
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_row_mid_c, cudaFuncAttributeMaxDynamicSharedMemorySize, smax);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_row_mid_fused_c, cudaFuncAttributeMaxDynamicSharedMemorySize, smax);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_hczt_row, cudaFuncAttributeMaxDynamicSharedMemorySize, smax);
     if (e != cudaSuccess) { d4w_row_plan_destroy(p); return fail(D4W_ERR_CUDA, std::string("row plan: ") + cudaGetErrorString(e)); }
     p->row.tw = p->d_tw; p->row.twT = p->d_twT;
@@ -159,8 +158,8 @@ extern "C" int d4w_row_plan_create(d4w_row_plan** out, int ns, int device) {
     cudaDeviceProp prop;
     D4W_CUDA_TRY(cudaGetDeviceProperties(&prop, device));
     FkHostPlan hp; std::string err;
-    // the envelope keeps k_row_mid_fused: 10 000 x 120 000 on an H100 took 15.5 ms with it and 16.9 ms with k_row_mid
-    // (two rows per transform both ways; one row per transform, no longer built: 25.1 ms)
+    // the envelope uses k_row_mid_fused: 10 000 x 120 000 on an H100 (700 W) took 13.7 ms with its per-pair kernels, 14.4 ms
+    // with the earlier spilling one (400 W card: 15.5 ms, against 16.9 ms with k_row_mid)
     // a length with no T1 x T2 split (a prime factor > 61, or T2 too long) goes through the chirp-z rows
     if (build_fk_hostplan(1, ns, prop.sharedMemPerBlockOptin, hp, err, /*allow_row_dual=*/false, /*row_fused_default=*/1))
         return row_plan_create_czt(out, ns, device, prop);
@@ -191,7 +190,6 @@ extern "C" int d4w_row_plan_create(d4w_row_plan** out, int ns, int device) {
     if (e == cudaSuccess) e = upload(&p->d_hilbert, h);
     if (e == cudaSuccess && !sg.empty()) e = upload(&p->d_sgn, sg);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_row_mid, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_row_mid_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_hilbert_row, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin);
     if (e != cudaSuccess) { d4w_row_plan_destroy(p); return fail(D4W_ERR_CUDA, std::string("row plan: ") + cudaGetErrorString(e)); }
     p->row.tw = p->d_tw; p->row.twT = p->d_twT;
@@ -237,20 +235,20 @@ static int hilbert_czt(d4w_row_plan* p, const float* x, float* out, int nx, void
     float2* w = (float2*)workspace;
     const int npair = (nx + 1) / 2, thr = 128;
     const dim3 g((p->t2 + thr - 1) / thr, npair), gm(p->t1, npair);
-    auto mid = [&](const float2* tab) {
-        if (p->fused) k_row_mid_fused_c<<<gm, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->czt_m, tab, (size_t)0);
-        else k_row_mid_c<<<gm, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->czt_m, tab, (size_t)0);
+    auto mid = [&](const float2* tab) -> int {
+        if (p->fused) return launch_row_mid_fused(gm, 256, p->row_smem, p->row, w, (size_t)p->czt_m, tab, 0, nullptr, p->device, stream);
+        k_row_mid_c<<<gm, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->czt_m, tab, (size_t)0);
+        D4W_CHECK_LAUNCH("k_row_mid_c");
+        return D4W_OK;
     };
     const int rc = with_t1(p->t1, [&](auto tc) -> int {
         constexpr int T1 = decltype(tc)::value;
         k_hczt_fwd<T1><<<g, thr, 0, stream>>>(hz, x, w);
         D4W_CHECK_LAUNCH("k_hczt_fwd");
-        mid(p->d_bhat);
-        D4W_CHECK_LAUNCH("k_row_mid_c");
+        if (const int r = mid(p->d_bhat)) return r;
         k_hczt_turn<T1><<<g, thr, 0, stream>>>(hz, w);
         D4W_CHECK_LAUNCH("k_hczt_turn");
-        mid(p->d_bhatc);
-        D4W_CHECK_LAUNCH("k_row_mid_c");
+        if (const int r = mid(p->d_bhatc)) return r;
         k_hczt_inv<T1><<<g, thr, 0, stream>>>(hz, w, x, out, mode, dev_stats);
         D4W_CHECK_LAUNCH("k_hczt_inv");
         return D4W_OK;
@@ -281,9 +279,13 @@ extern "C" int d4w_hilbert(d4w_row_plan* p, const float* x, float* out, int nx, 
         constexpr int T1 = decltype(tc)::value;
         k_hsplit_fwd2<T1><<<g, thr, 0, stream>>>(x, nx, p->ns, w, p->t2, p->d_twT);
         D4W_CHECK_LAUNCH("k_hsplit_fwd2");
-        if (p->fused) k_row_mid_fused<<<gm, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->ns, p->d_sgn, (size_t)0);
-        else k_row_mid<<<gm, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->ns, p->d_sgn, (size_t)0);
-        D4W_CHECK_LAUNCH("k_row_mid");
+        if (p->fused) {
+            if (const int r = launch_row_mid_fused(gm, 256, p->row_smem, p->row, w, (size_t)p->ns, p->d_sgn, 0, nullptr, p->device, stream))
+                return r;
+        } else {
+            k_row_mid<<<gm, 256, p->row_smem, stream>>>(p->row, w, (size_t)p->ns, p->d_sgn, (size_t)0);
+            D4W_CHECK_LAUNCH("k_row_mid");
+        }
         k_hsplit_inv2<T1><<<g, thr, 0, stream>>>(w, x, nx, p->ns, out, p->t2, p->d_twT, mode, dev_stats);
         D4W_CHECK_LAUNCH("k_hsplit_inv2");
         return D4W_OK;

@@ -165,6 +165,25 @@ __host__ __device__ inline void fft_inverse_stages(float2* s, const FftPlan& pl,
     }
 }
 
+// (first, last) radix of every row plan whose middle pass runs as k_row_mid_fused: one kernel per pair, so each holds
+// only its own butterflies (a run-time choice among all in-register radices spills at 128 registers).  The pairs are
+// those build_fk_hostplan gives split rows (T1 > 1) of every 2^a 3^b 5^c length up to 25 x 10 240 -- every f-k,
+// Hilbert and chirp-z row length with an in-register first and last stage; tests/test_row_fused_host.py re-derives
+// the list from the planner.  A plan whose pair is not listed uses k_row_mid.
+#define D4W_ROW_FUSED_PAIRS(X)                                                                                    \
+    X(3, 3) X(6, 3) X(6, 5) X(6, 15) X(8, 15) X(10, 15) X(10, 25) X(12, 3) X(12, 5) X(15, 3) X(16, 3) X(16, 5)   \
+    X(16, 8) X(16, 25) X(20, 15) X(20, 25) X(25, 5) X(25, 15)
+
+// f(integral_constant R0, integral_constant RL) for a listed pair; false (f not called) for any other
+template <class F>
+__host__ __device__ inline bool with_row_fused_pair(int r0, int rl, F&& f) {
+#define D4W_PAIR(A, B)                                                                        \
+    if (r0 == A && rl == B) { f(std::integral_constant<int, A>{}, std::integral_constant<int, B>{}); return true; }
+    D4W_ROW_FUSED_PAIRS(D4W_PAIR)
+#undef D4W_PAIR
+    return false;
+}
+
 // position -> frequency index after the forward transform (host side table builder)
 inline int pos_to_freq(const FftPlan& pl, int p) {
     int k = 0, mult = 1, rem = p, len = pl.n;

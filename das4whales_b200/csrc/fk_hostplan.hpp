@@ -122,7 +122,7 @@ inline const std::vector<int>& split_radices() {
 // returns 0 on success; 1 = unsupported shape (err says why)
 // row_fused_default: whether the middle row pass uses k_row_mid_fused unless D4W_ROW_FUSED says otherwise
 inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, std::string& err, bool allow_row_dual = true,
-                             int row_fused_default = 0) {
+                             int row_fused_default = 1) {
     hp.nx = nx; hp.ns = ns;
     const int col_maxr = env_int("D4W_COL_MAX_RADIX", 25);
     const int row_maxr = env_int("D4W_ROW_MAX_RADIX", 25);
@@ -313,10 +313,9 @@ inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, st
     hp.pos2k_row_tab = hp.pos2k_row;
     {
         const int nst = hp.rowpl.nstages;
-        auto inreg = [](int r) { for (int q : inreg_radices()) if (q == r) return true; return false; };
-        // f-k filter (default 0): on sm_90 k_row_mid_fused spills at its 128-register cap, and P3 ran 8.6 ms against 2.3 ms
-        // for k_row_mid (H100); the Hilbert plan passes 1, see d4w_row_plan_create
-        if (!hp.row_dual && env_int("D4W_ROW_FUSED", row_fused_default) && nst >= 2 && inreg(hp.rowpl.radix[0]) && inreg(hp.rowpl.radix[nst - 1])) {
+        // k_row_mid_fused is built for the (first, last) radix pairs of D4W_ROW_FUSED_PAIRS; other plans use k_row_mid
+        if (!hp.row_dual && env_int("D4W_ROW_FUSED", row_fused_default) && nst >= 2 &&
+            with_row_fused_pair(hp.rowpl.radix[0], hp.rowpl.radix[nst - 1], [](auto, auto) {})) {
             hp.row_fused = 1;
             const int rl = hp.rowpl.radix[nst - 1], G = hp.t2 / rl;
             for (int m = 0; m < rl; ++m)

@@ -15,6 +15,8 @@
 // per-thread loops are `for (i = tid; i < n; i += nthr)`, so tests/host_emul runs the very
 // same code on the CPU with nthr = 1.
 #pragma once
+#include <cstdio>
+#include <cstdlib>
 #include "fft_smem.cuh"
 #include "fft_dual.cuh"
 
@@ -1065,35 +1067,38 @@ __host__ __device__ inline void row_last_masked(float2* __restrict__ s, const Ta
 __host__ __device__ inline bool row_radix_inreg(int r) {
     return r == 2 || r == 3 || r == 4 || r == 5 || r == 6 || r == 8 || r == 10 || r == 12 || r == 15 || r == 16 || r == 20 || r == 25;
 }
-template <typename TabT, bool OOP = false>
+// R0 = rp.pl.radix[0], RL = rp.pl.radix[nstages - 1], fixed at compile time (D4W_ROW_FUSED_PAIRS)
+template <int R0, int RL, typename TabT, bool OOP = false>
 __host__ __device__ inline void body_row_mid_fused(const RowParams& rp, float2* __restrict__ w, size_t ldw,
                                                    const TabT* __restrict__ tab, size_t tab_slot_stride, int kt1, int slot,
                                                    int tid, int nthr, float2* smem, float2* __restrict__ dst = nullptr) {
     const int n = rp.t2, nst = rp.pl.nstages;
     float2* g = w + (size_t)slot * ldw + (size_t)kt1 * n;
     const TabT* m = tab + (size_t)slot * tab_slot_stride + (size_t)kt1 * n;
-    const int r0 = rp.pl.radix[0], rl = rp.pl.radix[nst - 1];
-#define D4W_CALL(R) row_first_fwd<R>(g, smem, rp.tw, n, tid, nthr);
-    D4W_ROW_RADIX_SWITCH(r0, D4W_CALL)
-#undef D4W_CALL
+    row_first_fwd<R0>(g, smem, rp.tw, n, tid, nthr);
     D4W_SYNC();
     fft_forward_stages(smem, rp.pl, rp.tw, 1, n, tid, nthr, 1, nst - 1);
-#define D4W_CALL(R) row_last_masked<R>(smem, m, n, tid, nthr);
-    D4W_ROW_RADIX_SWITCH(rl, D4W_CALL)
-#undef D4W_CALL
+    row_last_masked<RL>(smem, m, n, tid, nthr);
     D4W_SYNC();
     fft_inverse_stages(smem, rp.pl, rp.tw, 1, n, tid, nthr, 1, nst - 1);
-    if constexpr (OOP) {
-        float2* o = dst + (size_t)slot * ldw + (size_t)kt1 * n;
-#define D4W_CALL(R) row_first_inv<R>(o, smem, rp.tw, n, tid, nthr);
-        D4W_ROW_RADIX_SWITCH(r0, D4W_CALL)
-#undef D4W_CALL
-    } else {
-#define D4W_CALL(R) row_first_inv<R>(g, smem, rp.tw, n, tid, nthr);
-        D4W_ROW_RADIX_SWITCH(r0, D4W_CALL)
-#undef D4W_CALL
-    }
+    row_first_inv<R0>(OOP ? dst + (size_t)slot * ldw + (size_t)kt1 * n : g, smem, rp.tw, n, tid, nthr);
 }
+// host emulation: the same body with the plan's pair chosen at run time
+template <typename TabT, bool OOP = false>
+inline void body_row_mid_fused(const RowParams& rp, float2* w, size_t ldw, const TabT* tab, size_t tab_slot_stride, int kt1,
+                               int slot, int tid, int nthr, float2* smem, float2* dst = nullptr) {
+    const bool built = with_row_fused_pair(rp.pl.radix[0], rp.pl.radix[rp.pl.nstages - 1], [&](auto r0, auto rl) {
+        body_row_mid_fused<decltype(r0)::value, decltype(rl)::value, TabT, OOP>(rp, w, ldw, tab, tab_slot_stride, kt1, slot, tid,
+                                                                                 nthr, smem, dst);
+    });
+    if (!built) { fprintf(stderr, "body_row_mid_fused: no kernel for this plan's first / last radix\n"); abort(); }
+}
+#ifdef __CUDACC__
+// k_row_mid_fused for rp's pair (d4w_row_fused.cu); dst != nullptr (float table only): write the result there, w untouched
+template <typename TabT>
+int launch_row_mid_fused(dim3 grid, int threads, size_t smem, const RowParams& rp, float2* w, size_t ldw, const TabT* tab,
+                         size_t tab_slot_stride, float2* dst, int device, cudaStream_t stream);
+#endif
 
 // ================================================================== __global__ wrappers
 #ifdef __CUDACC__
@@ -1375,11 +1380,6 @@ k_row_split(float2* __restrict__ w, size_t ldw, int t2len, const float2* __restr
 static __global__ void __launch_bounds__(256, 2)
 k_row_mid(RowParams rp, float2* __restrict__ w, size_t ldw, const float* __restrict__ tab, size_t tab_slot_stride) {
     body_row_mid(rp, w, ldw, tab, tab_slot_stride, blockIdx.x, blockIdx.y, threadIdx.x, blockDim.x, d4w_dyn_smem);
-}
-
-static __global__ void __launch_bounds__(256, 2)
-k_row_mid_fused(RowParams rp, float2* __restrict__ w, size_t ldw, const float* __restrict__ tab, size_t tab_slot_stride) {
-    body_row_mid_fused(rp, w, ldw, tab, tab_slot_stride, blockIdx.x, blockIdx.y, threadIdx.x, blockDim.x, d4w_dyn_smem);
 }
 
 static __global__ void __launch_bounds__(128, 2)     // radix-25 dual butterflies need ~190 registers: 2 x 128-thread CTAs per SM

@@ -150,15 +150,10 @@ __host__ __device__ inline void body_hczt_inv(const HcztParams& hp, const float2
 }
 
 #ifdef __CUDACC__
-// the direct rows' middle passes with a complex table (B^ or conj B^)
+// the direct rows' middle pass with a complex table (B^ or conj B^); the fused one is in d4w_row_fused.cu
 static __global__ void __launch_bounds__(256, 2)
 k_row_mid_c(RowParams rp, float2* __restrict__ w, size_t ldw, const float2* __restrict__ tab, size_t tab_slot_stride) {
     body_row_mid(rp, w, ldw, tab, tab_slot_stride, blockIdx.x, blockIdx.y, threadIdx.x, blockDim.x, d4w_dyn_smem);
-}
-
-static __global__ void __launch_bounds__(256, 2)
-k_row_mid_fused_c(RowParams rp, float2* __restrict__ w, size_t ldw, const float2* __restrict__ tab, size_t tab_slot_stride) {
-    body_row_mid_fused(rp, w, ldw, tab, tab_slot_stride, blockIdx.x, blockIdx.y, threadIdx.x, blockDim.x, d4w_dyn_smem);
 }
 
 static __global__ void __launch_bounds__(256, 2)
