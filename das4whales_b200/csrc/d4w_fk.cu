@@ -200,7 +200,9 @@ extern "C" int d4w_fk_plan_create(d4w_fk_plan** out, int nx, int ns, int device)
         if (hp.pipe) {
             PipeParams& pp = pl->pipe;
             pp.nchunks = (ns / 2 + hp.chunk_pairs - 1) / hp.chunk_pairs;
-            pp.lag = hp.pipe_lag; pp.nbuf = hp.pipe_lag + std::max(2, env_int("D4W_PIPE_SLACK", 2));
+            // three ring slots beyond the lag (5 chunks, 33 MB of V at 10 000 channels, still inside the 50 MB L2): a producer
+            // waits less often for the consumers of the slot it re-uses; measured on the H100 against two, P1 5.08 -> 4.97 ms
+            pp.lag = hp.pipe_lag; pp.nbuf = hp.pipe_lag + std::max(2, env_int("D4W_PIPE_SLACK", 3));
             pp.cq = hp.pipe_cq; pp.rpc = (hp.fused3 ? hp.colb_threads : 160) / hp.pipe_cq;
             pp.nA = (hp.x2 + pp.rpc - 1) / pp.rpc;
             pp.tiles = hp.chunk_pairs / hp.np2; pp.nB = hp.planes * pp.tiles;
@@ -501,7 +503,11 @@ static int launch_col2_pipe(const d4w_fk_plan* pl, const d4w_fk_mask* m, const f
         D4W_CHECK_LAUNCH("k_col3_pipe");
         return D4W_OK;
     }
-    const int occ = env_int("D4W_PIPE_OCC", 3);       // CTAs per SM the kernel is compiled for: 3 = 128 registers (default), 4 = 96 (spills), 2 = 200
+    // CTAs per SM the kernel is compiled for: 3 = 128 registers, 4 = 96 (spills), 2 = 200.  Only 25 x (20 x 20) is built at
+    // 2 and 4; other splits run at 3.  The forward 25 x (20 x 20) kernel runs at 2: capped at 128 registers it spills, at 2
+    // CTAs/SM it takes 158 and none, and P1 at 10 000 x 120 000 fell from 5.50 to 5.08 ms on the H100.  The inverse takes
+    // 128 registers either way and runs at 3 (4.40 ms at both)
+    const int occ = env_int("D4W_PIPE_OCC", INV ? 3 : 2);
 #define D4W_PIPE_OCC(X1, RA, RB, OCC)                                                                                     \
     if (!done && x1 == X1 && ra == RA && occ == OCC) {                                                                    \
         static bool attr_done_dev[64] = {};                                                                               \

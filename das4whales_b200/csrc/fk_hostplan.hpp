@@ -275,9 +275,9 @@ inline int build_fk_hostplan(int nx, int ns, size_t smem_cap, FkHostPlan& hp, st
             // pipelined single launch: needs the fused level B with (ra, rb) in {(20,20), (16,25)} and 8-pair tiles
             if (env_int("D4W_COL_PIPE", 1) && hp.fused_ra && np == 8 &&
                 ((hp.fused_ra == 20 && hp.fused_rb == 20) || (hp.fused_ra == 16 && hp.fused_rb == 25))) {
-                // strip width in quads; 160 threads = cq x rpc.  40 keeps the 4-chunk V ring (13 planes x 400 x 80 pairs x 16 B
-                // = 6.7 MB per chunk, 27 MB in all at 10 000 channels) inside the H100's 50 MB L2; 80 (13.3 MB chunks, a 53 MB
-                // ring) measured 10 % slower
+                // strip width in quads; 160 threads = cq x rpc.  40 keeps the 5-chunk V ring (13 planes x 400 x 80 pairs x 16 B
+                // = 6.7 MB per chunk, 33 MB in all at 10 000 channels) inside the H100's 50 MB L2; 80 (13.3 MB chunks, a 53 MB
+                // ring of 4) measured 10 % slower
                 int cq = env_int("D4W_PIPE_CQ", 40);
                 if (cq < 4 || 160 % cq || (2 * cq) % np) cq = 40;
                 hp.pipe = 1; hp.pipe_cq = cq; hp.chunk_pairs = 2 * cq;
