@@ -11,5 +11,5 @@ keeps the `das4whales.dsp` / `das4whales.detect` signatures (reference:
 """
 __version__ = "0.1.0"
 
-from . import dsp, detect, fk, data_handle, improcess, tools  # noqa: F401
+from . import dsp, detect, fk, data_handle, improcess, tools, loc  # noqa: F401
 from ._build import build_library  # noqa: F401

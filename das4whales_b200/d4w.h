@@ -297,6 +297,26 @@ int d4w_filter2d(const float* dev_in, int h, int w, const float* dev_K, int kh, 
                  float* dev_out, void* stream);
 int d4w_mask_upsample_mul(const float* dev_trace, int nx, int ns, const float* dev_mask, int mh, int mw, float* dev_out,
                           unsigned char* dev_mask_out, void* stream);
+/* ---- localisation: loc.solve_lq, loc.calc_covariance_matrix, loc.calc_uncertainty_position (das4whales/loc.py:57-216) for
+ *      a batch of calls, in FP64.  Call b is the observations [dev_offsets[b], dev_offsets[b + 1]) of dev_T (arrival times, s)
+ *      and dev_pos ([n_obs][3], m); p = 4 unknowns (x, y, z, t0), or 3 with fix_z (z held at the first guess).
+ *  d4w_loc_grid: first guess from a grid search.  Nodes (dev_gx[ix], dev_gy[iy], dev_gz[iz]), index (iz * ny + iy) * nx + ix;
+ *      score = sum (T - t0* - d / c0)^2 / (n - p), t0* = mean(T - d / c0).  dev_index[b] (int64) = the node of least score
+ *      (ties to the lowest index), dev_score[b] (NaN when n <= p), dev_n0[b][4] = (node, t0*); an empty call gets index -1
+ *      and NaN.  fix_z needs nz = 1.  dev_workspace: d4w_loc_grid_workspace_bytes bytes.
+ *  d4w_loc_solve: Nbiter Gauss-Newton steps from dev_n0[b][4] (NULL: the reference's [40000, 23000, -60, min T]) with
+ *      (G^T G + 1e-5 I) dn = G^T dt and a step of 0.7 dn for the first four; then dev_n[b][4], dev_var[b] = sum dt^2 / (n - p)
+ *      (NaN when n <= p), C = (G^T G)^-1 at the final n, or (G^T G + 1e-5 I)^-1 when its 2-norm condition number exceeds
+ *      1 / DBL_EPSILON, and dev_unc[b][p] = sqrt(var diag C).  Optional (NULL to skip): dev_cinv[b][p][p] = C,
+ *      dev_cond[b], dev_traj[b][nbiter][4] the estimate after every iteration, dev_n0_used[b][4] the first guess.  An empty
+ *      call is NaN throughout.  Deterministic: no atomics, fixed reduction order. */
+size_t d4w_loc_grid_workspace_bytes(int ncalls, int nx, int ny, int nz);
+int d4w_loc_grid(const double* dev_T, const double* dev_pos, const long long* dev_offsets, int ncalls, double c0, int fix_z,
+                 const double* dev_gx, int nx, const double* dev_gy, int ny, const double* dev_gz, int nz, void* dev_workspace,
+                 long long* dev_index, double* dev_score, double* dev_n0, void* stream);
+int d4w_loc_solve(const double* dev_T, const double* dev_pos, const long long* dev_offsets, int ncalls, double c0, int nbiter,
+                  int fix_z, const double* dev_n0, double* dev_n, double* dev_var, double* dev_unc, double* dev_cinv,
+                  double* dev_cond, double* dev_traj, double* dev_n0_used, void* stream);
 /* D4W_CDEF_END */
 
 #ifdef __cplusplus
