@@ -317,6 +317,24 @@ int d4w_loc_grid(const double* dev_T, const double* dev_pos, const long long* de
 int d4w_loc_solve(const double* dev_T, const double* dev_pos, const long long* dev_offsets, int ncalls, double c0, int nbiter,
                   int fix_z, const double* dev_n0, double* dev_n, double* dev_var, double* dev_unc, double* dev_cinv,
                   double* dev_cond, double* dev_traj, double* dev_n0_used, void* stream);
+
+/* ---- image operators of improcess outside the Gabor path (das4whales/improcess.py:143-169, :319-367).
+ *  d4w_radon: skimage.transform.radon(image, theta, circle=False) of the float32 image [h][w] placed at rows
+ *      [pad_r, pad_r + h), columns [pad_c, pad_c + w) of an n x n zero square.  dev_cs: double [nangles][2] = (cos, sin) of
+ *      each angle; dev_out: double [n][nangles], bin b at angle a = the sum over rows r of the bilinear sample of the square
+ *      at x = cos b + sin r - c (cos + sin - 1), y = -sin b + cos r - c (cos - sin - 1), c = n / 2.  No atomics: runs are
+ *      bit-identical.
+ *  d4w_bilateral: cv2.bilateralFilter(img, 2 radius + 1, sigma_color, sigma_space) of one channel, with the
+ *      caller's radius (1..64) and sigmas (> 0) already normalised as OpenCV does.  is_8u: the image holds the integers of an
+ *      8-bit image and the result is rounded and saturated to them; otherwise 32F.  dev_workspace: D4W_BILATERAL_WS_BYTES.
+ *  d4w_grad_oriented: improcess.gradient_oriented(image, (dft, dfx)) for dft, dfx >= 0, not both 0: dev_out is
+ *      [h][w - dft] (dfx = 0), [h - dfx][w] (dft = 0) or [h - 2 dfx][w - dft]; an empty output is D4W_ERR_ARG. */
+enum { D4W_BILATERAL_WS_BYTES = 16 + 4 * 4099 };
+int d4w_radon(const float* dev_img, int h, int w, int n, int pad_r, int pad_c, const double* dev_cs, int nangles,
+              double* dev_out, void* stream);
+int d4w_bilateral(const float* dev_in, int h, int w, int is_8u, int radius, double sigma_color, double sigma_space,
+                  void* dev_workspace, float* dev_out, void* stream);
+int d4w_grad_oriented(const float* dev_in, int h, int w, int dft, int dfx, float* dev_out, void* stream);
 /* D4W_CDEF_END */
 
 #ifdef __cplusplus

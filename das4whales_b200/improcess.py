@@ -4,8 +4,10 @@ Drop-in for the functions of `das4whales.improcess` that scripts/main_gabordetec
 (/root/reference/src/das4whales/improcess.py): scale_pixels (:23-41), trace2image (:44-63), angle_fromspeed (:66-95),
 gabor_filt_design (:98-140), binning (:395-421), apply_smooth_mask (:424-454); plus `filter2D`, the GPU stand-in for the
 `cv2.filter2D(img, cv2.CV_64F, kernel)` calls the script makes (:109, :135), and `gabor_detect`, which chains the whole
-script section :78-169 on the device.  Everything numeric runs in libd4w.so (csrc/image_kernels.cuh); OpenCV / torchvision
-are not used.
+script section :78-169 on the device.  The reference's other image operators follow at the end: compute_radon_transform
+(:347), bilateral_filter (:319), gaussian_filter (:370), detect_diagonal_edges (:172), diagonal_edge_detection (:229) and
+gradient_oriented (:143) (csrc/imageops_kernels.cuh and filter2D).  Everything numeric runs in libd4w.so
+(csrc/image_kernels.cuh); OpenCV / torchvision / skimage are not used.
 
 ndarray in -> float64 ndarray out (like the reference); CUDA tensor in -> float32 CUDA tensor out.
 """
@@ -192,3 +194,200 @@ def gabor_detect(trf_fk, fs, dx, selected_channels, c0=1500., bin_factor=10, thr
         return res
     conv = (lambda t: t) if _is_tensor(trf_fk) else (lambda t: t.to(torch.float64).cpu().numpy())
     return res, {"image": conv(image), "imagebin": conv(imagebin), "fimage": conv(fimage), "mask": conv(mask) != 0}
+
+
+# ------------------------------------------------------------------------------ the operators outside the Gabor path
+# improcess.py:143-169, :172-266, :319-392 of the reference.  Arguments are checked on the host before any device work.
+def _dtype_name(img):
+    """numpy-style name of an ndarray's or a tensor's dtype ('uint8', 'float32', ...)"""
+    return str(img.dtype).split(".")[-1] if _is_tensor(img) else np.asarray(img).dtype.name
+
+
+def _check_image(img, what):
+    """(image as ndarray or tensor, dtype name) of a non-empty 2-D real image; ValueError otherwise"""
+    if not _is_tensor(img):
+        img = np.asarray(img)
+    name = _dtype_name(img)
+    if img.ndim != 2 or img.shape[0] < 1 or img.shape[1] < 1:
+        raise ValueError(f"{what}: expected a non-empty 2-D image, got shape {tuple(img.shape)}")
+    if name not in ("bool", "uint8", "uint16", "int8", "int16", "int32", "int64", "float16", "float32", "float64"):
+        raise ValueError(f"{what}: unsupported dtype {name}")
+    return img, name
+
+
+def _as_int(v, what):
+    try:
+        i = int(v)
+    except (TypeError, ValueError):
+        raise ValueError(f"{what} must be an integer") from None
+    if i != v:
+        raise ValueError(f"{what} must be an integer")
+    return i
+
+
+def _as_real(v, what):
+    try:
+        f = float(v)
+    except (TypeError, ValueError):
+        raise ValueError(f"{what} must be a real number") from None
+    if not np.isfinite(f):
+        raise ValueError(f"{what} must be finite")
+    return f
+
+
+def _out(y, like):
+    return y if _is_tensor(like) else _to_host64(y)
+
+
+# skimage's img_as_float: the integer scale of each accepted dtype
+_RADON_SCALE = {"bool": 1.0, "uint8": 255.0, "uint16": 65535.0, "float16": 1.0, "float32": 1.0, "float64": 1.0}
+
+
+def _radon_square(h, w):
+    """(n, pad_rows, pad_cols): skimage's radon(circle=False) zero-pads an h x w image to an n x n square,
+    n = ceil(sqrt(2) max(h, w)), with (s + p) // 2 - s // 2 of the p = n - s padding rows / columns before the image."""
+    diagonal = np.sqrt(2) * max(h, w)
+    pad = [int(np.ceil(diagonal - s)) for s in (h, w)]
+    before = [(s + p) // 2 - s // 2 for s, p in zip((h, w), pad)]
+    return h + pad[0], before[0], before[1]
+
+
+def compute_radon_transform(image, theta=None):
+    """skimage.transform.radon(image, theta, circle=False) (reference: improcess.py:347-367): the sum of every column of
+    the padded image rotated by each angle (degrees, default 0..179), bilinear, zero outside.  Returns [n, len(theta)],
+    n = ceil(sqrt(2) max(h, w)).  uint8 / uint16 / bool images are scaled as skimage.img_as_float scales them; other integer
+    dtypes raise ValueError.  Ray sums run in double on the GPU (d4w_radon), so the result does not depend on the launch."""
+    image, name = _check_image(image, "compute_radon_transform")
+    if name not in _RADON_SCALE:
+        raise ValueError(f"compute_radon_transform: unsupported dtype {name} (skimage.img_as_float takes floats, uint8, uint16, bool)")
+    th = np.arange(180) if theta is None else theta
+    try:
+        th = np.asarray(th.cpu() if _is_tensor(th) else th, dtype=np.float64)
+    except (TypeError, ValueError):
+        raise ValueError("compute_radon_transform: theta must be a 1-D array of angles in degrees") from None
+    if th.ndim != 1 or th.size < 1 or not np.all(np.isfinite(th)):
+        raise ValueError("compute_radon_transform: theta must be a 1-D array of at least one finite angle")
+    h, w = image.shape
+    n, pad_r, pad_c = _radon_square(h, w)
+    angles = np.deg2rad(th)
+    cs = np.ascontiguousarray(np.stack([np.cos(angles), np.sin(angles)], axis=1))
+    torch = _torch()
+    x = _dev2d(image)
+    dcs = torch.from_numpy(cs).to(x.device)
+    out = torch.empty((n, th.size), dtype=torch.float64, device=x.device)
+    with torch.cuda.device(x.device.index):
+        _lib.check(_lib.lib().d4w_radon(_lib.ptr(x, "float*"), h, w, n, pad_r, pad_c, _lib.ptr(dcs, "double*"), th.size,
+                                        _lib.ptr(out, "double*"), _lib.stream_ptr()), "compute_radon_transform")
+    if _RADON_SCALE[name] != 1.0:
+        out /= _RADON_SCALE[name]          # the transform is linear: scaling the sums is img_as_float's scaling, exactly
+    return out.to(torch.float32) if _is_tensor(image) else out.cpu().numpy()
+
+
+def bilateral_filter(img, diameter, sigma_color, sigma_space):
+    """cv2.bilateralFilter(img, diameter, sigma_color, sigma_space) of a single-channel uint8 or float32 image (reference:
+    improcess.py:319-344; cv2 rejects other depths, so they raise ValueError here).  OpenCV's rules, as cv2 4.13 applies
+    them: either sigma <= 0 returns the image unchanged, for both depths; the radius is round(1.5 sigma_space) for
+    diameter <= 0, diameter // 2 otherwise, at least 1 (here at most 64); the taps are those within the radius, border
+    reflect-101; uint8 weighs colours by an exact table and rounds the result, float32 by a 4 096-bin table over the image's
+    range (colour weight 1 throughout for a constant image).  The result holds the uint8 values for a uint8 image (float64 /
+    float32 out, as the rest of the module)."""
+    img, name = _check_image(img, "bilateral_filter")
+    if name not in ("uint8", "float32"):
+        raise ValueError(f"bilateral_filter: OpenCV filters uint8 and float32 images only, got {name}")
+    d = _as_int(diameter, "bilateral_filter: diameter")
+    sc = _as_real(sigma_color, "bilateral_filter: sigma_color")
+    ss = _as_real(sigma_space, "bilateral_filter: sigma_space")
+    copy = sc <= 0 or ss <= 0                              # cv2 returns the image unchanged then
+    radius = 1 if copy else max(int(np.rint(ss * 1.5)) if d <= 0 else d // 2, 1)
+    if radius > 64:
+        raise ValueError(f"bilateral_filter: radius {radius} > 64 is not supported")
+    torch = _torch()
+    x = _dev2d(img)
+    if copy:
+        return _out(x.clone(), img)
+    h, w = x.shape
+    out = torch.empty_like(x)
+    ws = torch.empty(_lib.lib().D4W_BILATERAL_WS_BYTES, dtype=torch.uint8, device=x.device)
+    with torch.cuda.device(x.device.index):
+        _lib.check(_lib.lib().d4w_bilateral(_lib.ptr(x, "float*"), h, w, int(name == "uint8"), radius, sc, ss, _lib.ptr(ws),
+                                            _lib.ptr(out, "float*"), _lib.stream_ptr()), "bilateral_filter")
+    return _out(out, img)
+
+
+# OpenCV's getGaussianKernel uses fixed tables for sigma <= 0 and these sizes (checked against cv2 4.13, which also has 9)
+_GAUSS_TABLES = {1: [1.0], 3: [0.25, 0.5, 0.25], 5: [0.0625, 0.25, 0.375, 0.25, 0.0625],
+                 7: [0.03125, 0.109375, 0.21875, 0.28125, 0.21875, 0.109375, 0.03125],
+                 9: [4 / 256, 13 / 256, 30 / 256, 51 / 256, 60 / 256, 51 / 256, 30 / 256, 13 / 256, 4 / 256]}
+
+
+def _gaussian_kernel(size, sigma):
+    """cv2.getGaussianKernel(size, sigma) restated: a fixed table for sigma <= 0 and size <= 9, otherwise
+    exp(-x^2 / (2 s^2)) normalised to sum 1 over x = i - (size - 1) / 2, s = sigma, or ((size - 1) / 2 - 1) 0.3 + 0.8 for
+    sigma <= 0."""
+    if sigma <= 0 and size in _GAUSS_TABLES:
+        return np.array(_GAUSS_TABLES[size])
+    s = sigma if sigma > 0 else ((size - 1) * 0.5 - 1) * 0.3 + 0.8
+    x = np.arange(size) - (size - 1) * 0.5
+    t = np.exp(-0.5 / (s * s) * x * x)
+    return t / t.sum()
+
+
+def gaussian_filter(img, size, sigma):
+    """cv2.GaussianBlur(img, (size, size), sigma) (reference: improcess.py:370-392): one filter2D pass (reflect-101) with
+    the outer product of _gaussian_kernel(size, sigma).  `size` must be odd and positive.  An integer image is filtered as
+    its values; the result is not rounded back to the input depth."""
+    img, _ = _check_image(img, "gaussian_filter")
+    size = _as_int(size, "gaussian_filter: size")
+    if size < 1 or size % 2 == 0:
+        raise ValueError("gaussian_filter: size must be odd and positive")
+    g = _gaussian_kernel(size, _as_real(sigma, "gaussian_filter: sigma"))
+    return filter2D(img, None, np.outer(g, g))
+
+
+_DIAG5 = np.array([[0, 1, 1, 1, 1], [-1, 0, 1, 1, 1], [-1, -1, 0, 1, 1], [-1, -1, -1, 0, 1], [-1, -1, -1, -1, 0]], np.float64)
+_DIAG3 = np.array([[2, -1, -1], [-1, 2, -1], [-1, -1, 2]], np.float64)
+
+
+def detect_diagonal_edges(matrix, threshold):
+    """fftconvolve(matrix, K, 'same') + fftconvolve(matrix, fliplr(K), 'same') with the reference's 5 x 5 diagonal kernel K
+    (reference: improcess.py:172-226; `threshold` is unused there too).  A convolution is a correlation with the kernel
+    turned by 180 degrees, so this is one zero-border filter2D pass with rot180(K) + rot180(fliplr(K))."""
+    matrix, _ = _check_image(matrix, "detect_diagonal_edges")
+    return filter2D(matrix, None, _DIAG5[::-1, ::-1] + _DIAG5[::-1, :], border="zeros")
+
+
+def diagonal_edge_detection(img, threshold):
+    """conv2d(img, W, padding=1) + conv2d(img, flip(W, 0), padding=1) with the reference's 3 x 3 kernel W (reference:
+    improcess.py:229-266): one zero-border filter2D pass with W + flip(W, 0).  Returns what the reference returns, a
+    float32 torch tensor: on the CPU for an ndarray, on the input's device for a tensor."""
+    img, _ = _check_image(img, "diagonal_edge_detection")
+    y = filter2D(_dev2d(img), None, _DIAG3 + _DIAG3[::-1, :], border="zeros")
+    return y.to(img.device) if _is_tensor(img) else y.cpu()
+
+
+def gradient_oriented(image, direction):
+    """The reference's oriented difference (improcess.py:143-169) for shifts dft, dfx >= 0:
+    dfx = 0: -(x[:, :-dft] - x[:, dft:]); dft = 0: -(x[dfx:, :] - x[:-dfx, :]);
+    otherwise -(x[dfx:-dfx, :-dft] - 0.5 x[2 dfx:, dft:] - 0.5 x[:-2 dfx, dft:]).  (0, 0) raises ValueError, as the
+    reference's broadcast fails.  An integer image is taken as its values (no unsigned wrap-around)."""
+    image, _ = _check_image(image, "gradient_oriented")
+    try:
+        dft, dfx = direction
+    except (TypeError, ValueError):
+        raise ValueError("gradient_oriented: direction must be a pair (dft, dfx)") from None
+    dft, dfx = _as_int(dft, "gradient_oriented: dft"), _as_int(dfx, "gradient_oriented: dfx")
+    if dft < 0 or dfx < 0:
+        raise ValueError("gradient_oriented: dft and dfx must be >= 0")
+    if dft == 0 and dfx == 0:
+        raise ValueError("gradient_oriented: direction (0, 0) has no gradient (the reference's shapes do not broadcast)")
+    h, w = image.shape
+    oh = max(0, h if dfx == 0 else h - dfx if dft == 0 else h - 2 * dfx)
+    ow = max(0, w - dft)
+    torch = _torch()
+    x = _dev2d(image)
+    out = torch.empty((oh, ow), dtype=torch.float32, device=x.device)
+    if oh and ow:
+        with torch.cuda.device(x.device.index):
+            _lib.check(_lib.lib().d4w_grad_oriented(_lib.ptr(x, "float*"), h, w, dft, dfx, _lib.ptr(out, "float*"),
+                                                    _lib.stream_ptr()), "gradient_oriented")
+    return out if _is_tensor(image) else out.to(torch.float64).cpu().numpy()
