@@ -673,7 +673,7 @@ k_hsplit_inv2(const float2* __restrict__ w, const float* __restrict__ x, int nx,
         constexpr int j = decltype(jc)::value;
         const size_t o = (size_t)j * t2len;
         oa[o] = hilbert_epilogue2(xa[o], v[j].y, mode, va);
-        if (has_b) oa[ns + o] = hilbert_epilogue2(xa[ns + o], v[j].x, mode, vb);
+        if (has_b) oa[ns + o] = hilbert_epilogue2(xa[ns + o], -v[j].x, mode, vb);
     });
 }
 

@@ -14,8 +14,25 @@ pytestmark = pytest.mark.gpu
 FS = 200.0
 TOL = 1e-4
 # every one of these lengths has a prime factor > 61 (no direct plan); 8 191 / 8 193 sit on either side of the
-# whole-row (convolution <= 16 384 points) / split boundary
-LENGTHS = [751, 1126, 1501, 4099, 8191, 8193, 15001, 127997]
+# whole-row (convolution <= 16 384 points) / split boundary; from 16 933 on, one length per further split radix
+LENGTHS = [751, 1126, 1501, 4099, 8191, 8193, 15001, 127997,
+           16933, 16399, 19573, 30723, 31161, 39083, 41877, 61854, 62234, 8443]
+# T1 of the split lengths (convolution length M = T1 x T2 in the comments); every other length is a whole row (T1 = 1)
+SPLIT_T1 = {
+    8193: 3,        # 16 875
+    15001: 3,       # 30 375
+    127997: 25,     # 256 000
+    16933: 4,       # 34 560
+    16399: 5,       # 32 805
+    19573: 6,       # 39 366
+    30723: 8,       # 62 208
+    31161: 10,      # 62 500
+    39083: 12,      # 78 732
+    41877: 15,      # 84 375
+    61854: 16,      # 124 416
+    62234: 20,      # 125 000
+    8443: 2,        # 17 280
+}
 
 
 @pytest.fixture(scope="module")
@@ -81,6 +98,7 @@ def test_hilbert_family_czt_lengths(dw, fresh_plans, monkeypatch, env):
         t1, t2, m = plan.info()
         assert m >= 2 * n - 1 and t1 * t2 == m, (n, t1, t2, m)
         assert (t1 == 1) == (m <= 16384), (n, t1, m)
+        assert t1 == SPLIT_T1.get(n, 1), (n, t1)
         ws = _lib.lib().d4w_row_workspace_bytes(plan.ptr, nx)
         assert ws == (16 if t1 == 1 else (nx + 1) // 2 * m * 8), (n, ws)
 

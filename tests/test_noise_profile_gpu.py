@@ -81,6 +81,8 @@ CASES = [
     (2, 120000, 0, None, "split"),
     (3, 40000, 3000, 17000, "split"),                 # strided long window
     (3, 20000, 20000 - 16385, 16385, "split_czt"),    # strided long window ending at ns
+    (3, 16445, 0, None, "split"),                     # odd direct split: T1 = 5, T2 = 11 * 13 * 23
+    (2, 30723, 0, None, "split_czt"),                 # chirp-z split with T1 = 8
 ]
 
 
