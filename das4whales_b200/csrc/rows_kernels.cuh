@@ -338,9 +338,9 @@ k_xcorr_fused(XcorrParams xp, const float* __restrict__ x, const float2* __restr
 // signal a + i b, lane B is c + i d, and both lanes run through one instruction stream of butterflies whose twiddles are
 // formed once for the two lanes (each lane operation is a scalar FFMA / FADD / FMUL, fft_dual.cuh).
 // The template spectra are lane-independent scalars (dmul_s).  Shared memory: S and B as cpd (16 B x nb each) and the
-// exclusive prefix sums of the mu term as a coarse float4 per 8 samples + an fp16 x 4 remainder per sample (the remainder is
-// a sum of <= 7 normalised samples, |.| <= 7, so its fp16 rounding is <= 4e-3 before the ~1e-6 factor mu / m).
-struct __align__(8) half4 { __half2 ac, bd; };
+// exclusive prefix sums of the mu term as a float4 per 8 samples; the output sweep adds the <= 7 samples before each output
+// in its group, re-read from the input in fp32 (an fp16 per-sample remainder in shared memory cost up to 3e-5 l2 error
+// when mu / m is large: short rows, templates with a large mean).
 
 template <int R>
 __device__ __forceinline__ void xcorrd_last_fused(const cpd* __restrict__ S, cpd* __restrict__ B, const float2* __restrict__ tab,
@@ -356,9 +356,9 @@ __device__ __forceinline__ void xcorrd_last_fused(const cpd* __restrict__ S, cpd
     }
 }
 template <int R>
-__device__ __forceinline__ void xcorrd_first_inv_out(const cpd* __restrict__ B, const float4* __restrict__ Pc, const half4* __restrict__ Pf,
-                                                     const float2* __restrict__ tw, int nb, int V, int t0, int ns, float mu, bool use_p,
-                                                     float* __restrict__ o, int tid, int nthr) {
+__device__ __forceinline__ void xcorrd_first_inv_out(const cpd* __restrict__ B, const float4* __restrict__ Pc, const float* __restrict__ r,
+                                                     float mean, float inv, const float2* __restrict__ tw, int nb, int V, int t0, int ns,
+                                                     float mu, bool use_p, float* __restrict__ o, int tid, int nthr) {
     const int L = nb / R;
     for (int n = tid; n < L; n += nthr) {
         cpd v[R];
@@ -371,13 +371,19 @@ __device__ __forceinline__ void xcorrd_first_inv_out(const cpd* __restrict__ B, 
             if (i < V) {
                 const cpd z = v[outpos<R>(q)];
                 float va = f2x_lo(z.x), vc = f2x_hi(z.x), vb = f2x_lo(z.y), vd = f2x_hi(z.y);
-                if (use_p) {
-                    const float4 c = Pc[i >> 3];
-                    const half4 f = Pf[i];
-                    const float2 fac = __half22float2(f.ac), fbd = __half22float2(f.bd);
-                    va += mu * (c.x + fac.x); vb += mu * (c.y + fbd.x); vc += mu * (c.z + fac.y); vd += mu * (c.w + fbd.y);
-                }
                 const int ta = t0 + i, tb = ta + V, tc = tb + V, td = tc + V;
+                if (use_p) {
+                    // exclusive prefix = group prefix + the <= 7 normalised samples before i in its group, re-read in fp32
+                    float4 c = Pc[i >> 3];
+                    for (int k = i & ~7; k < i; ++k) {
+                        const int ka = t0 + k, kb = ka + V, kc = kb + V, kd = kc + V;
+                        c.x += (ka < ns) ? (r[ka] - mean) * inv : 0.f;
+                        c.y += (kb < ns) ? (r[kb] - mean) * inv : 0.f;
+                        c.z += (kc < ns) ? (r[kc] - mean) * inv : 0.f;
+                        c.w += (kd < ns) ? (r[kd] - mean) * inv : 0.f;
+                    }
+                    va += mu * c.x; vb += mu * c.y; vc += mu * c.z; vd += mu * c.w;
+                }
                 if (ta < ns) o[ta] = va;
                 if (tb < ns) o[tb] = vb;
                 if (tc < ns) o[tc] = vc;
@@ -414,7 +420,6 @@ k_xcorr_dual(XcorrParams xp, const float* __restrict__ x, const float2* __restri
     cpd* S = reinterpret_cast<cpd*>(smraw);
     cpd* B = S + nb;
     float4* Pc = reinterpret_cast<float4*>(B + nb);
-    half4* Pf = reinterpret_cast<half4*>(Pc + ng);
     __shared__ float4 s_wsum[8];
     const int tid = threadIdx.x, nthr = blockDim.x, lane = tid & 31, wid = tid >> 5;
     const int row = blockIdx.y;
@@ -472,8 +477,6 @@ k_xcorr_dual(XcorrParams xp, const float* __restrict__ x, const float2* __restri
             Pc[g] = run;
             float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
             for (int i = g * 8; i < min(V, g * 8 + 8); ++i) {
-                half4 h; h.ac = __floats2half2_rn(f.x, f.z); h.bd = __floats2half2_rn(f.y, f.w);
-                Pf[i] = h;
                 const cpd z = S[i];
                 f.x += f2x_lo(z.x); f.y += f2x_lo(z.y); f.z += f2x_hi(z.x); f.w += f2x_hi(z.y);
             }
@@ -498,7 +501,7 @@ k_xcorr_dual(XcorrParams xp, const float* __restrict__ x, const float2* __restri
         }
         const float mu = (!SAME && xp.normalize) ? (float)mu_over_m[t] : 0.f;
         float* o = out + (size_t)t * out_tpl_stride + (size_t)row * ns;
-#define D4W_CALL(R) xcorrd_first_inv_out<R>(B, Pc, Pf, xp.tw, nb, V, t0, ns, mu, !SAME && xp.normalize != 0, o, tid, nthr);
+#define D4W_CALL(R) xcorrd_first_inv_out<R>(B, Pc, r, mean, inv, xp.tw, nb, V, t0, ns, mu, !SAME && xp.normalize != 0, o, tid, nthr);
         D4W_SMALL_RADIX_SWITCH(r0, D4W_CALL)
 #undef D4W_CALL
         __syncthreads();
@@ -509,6 +512,13 @@ k_xcorr_dual(XcorrParams xp, const float* __restrict__ x, const float2* __restri
 // but no twiddle factors between the stages and conflict-free strides.  The block is loaded in natural time order (B),
 // prefix-summed, scattered to the 4-D positions (S), transformed, and the result is gathered back to time order on the way out
 // so that every global access stays coalesced.  tabs[t][m * 280 + j] belongs to position j * 9 + m (d4w_fft_plan_table_order).
+// Exclusive prefix of the mu term in k_xcorr_pfa: a float4 per group of 8 samples (Pc) plus the in-group remainder per sample
+// in fp16 (Pf; an fp32 remainder would not fit two CTAs per SM).  The remainder is a sum of <= 7 normalised samples,
+// |.| <= 14, so its fp16 rounding is <= 7e-3 and costs <= 1e-7 on the output while |mu / m| <= 2^-16 -- the script's chirps
+// on rows of >= 1 500 samples.  Larger |mu / m| (templates with a visible mean, short rows) would see it (up to 3e-5 l2 with
+// a 300-tap Hann pulse on 400-sample rows): the output sweep then rebuilds the remainder in fp32 from the input instead.
+struct __align__(8) half4 { __half2 ac, bd; };
+constexpr float kXcorrMuFp16Max = 1.0f / 65536;
 constexpr int kPfaThreads = 256;      // measured: 256 threads 10.8 ms, 320 threads 11.2 ms (10 000 x 120 000, HF + LF)
 template <bool SAME>
 static __global__ void __launch_bounds__(kPfaThreads, 2)
@@ -598,20 +608,49 @@ k_xcorr_pfa(XcorrParams xp, const int* __restrict__ tpos, const float* __restric
         pfa_inverse_3(B, tid, nthr);
         const float mu = (!SAME && xp.normalize) ? (float)mu_over_m[t] : 0.f;
         float* o = out + (size_t)t * out_tpl_stride + (size_t)row * ns;
-        for (int i = tid; i < V; i += nthr) {
-            const cpd z = B[tpos[i]];
-            float va = f2x_lo(z.x), vc = f2x_hi(z.x), vb = f2x_lo(z.y), vd = f2x_hi(z.y);
-            if (!SAME && xp.normalize) {
-                const float4 c = Pc[i >> 3];
-                const half4 f = Pf[i];
-                const float2 fac = __half22float2(f.ac), fbd = __half22float2(f.bd);
-                va += mu * (c.x + fac.x); vb += mu * (c.y + fbd.x); vc += mu * (c.z + fac.y); vd += mu * (c.w + fbd.y);
+        if (!SAME && xp.normalize && fabsf(mu) > kXcorrMuFp16Max) {
+            for (int i0 = 0; i0 < V; i0 += nthr) {               // every lane runs every iteration (full-mask shuffles below)
+                // in-group exclusive prefix in fp32: the load sweep's segmented scan again, on the samples re-read from the
+                // input (L2-resident)
+                const int i = i0 + tid;
+                const int ta = t0 + i, tb = ta + V, tc = tb + V, td = tc + V;
+                const float a = (i < V && ta < ns) ? (r[ta] - mean) * inv : 0.f;
+                const float b = (i < V && tb < ns) ? (r[tb] - mean) * inv : 0.f;
+                const float c = (i < V && tc < ns) ? (r[tc] - mean) * inv : 0.f;
+                const float d = (i < V && td < ns) ? (r[td] - mean) * inv : 0.f;
+                float4 inc = make_float4(a, b, c, d);
+#pragma unroll
+                for (int s = 1; s < 8; s <<= 1) {
+                    const float ux = __shfl_up_sync(0xffffffffu, inc.x, s), uy = __shfl_up_sync(0xffffffffu, inc.y, s);
+                    const float uz = __shfl_up_sync(0xffffffffu, inc.z, s), uw = __shfl_up_sync(0xffffffffu, inc.w, s);
+                    if ((lane & 7) >= s) { inc.x += ux; inc.y += uy; inc.z += uz; inc.w += uw; }
+                }
+                if (i >= V) continue;
+                const float4 g = Pc[i >> 3];
+                const cpd z = B[tpos[i]];
+                const float va = f2x_lo(z.x) + mu * (g.x + inc.x - a), vb = f2x_lo(z.y) + mu * (g.y + inc.y - b);
+                const float vc = f2x_hi(z.x) + mu * (g.z + inc.z - c), vd = f2x_hi(z.y) + mu * (g.w + inc.w - d);
+                if (ta < ns) o[ta] = va;
+                if (tb < ns) o[tb] = vb;
+                if (tc < ns) o[tc] = vc;
+                if (td < ns) o[td] = vd;
             }
-            const int ta = t0 + i, tb = ta + V, tc = tb + V, td = tc + V;
-            if (ta < ns) o[ta] = va;
-            if (tb < ns) o[tb] = vb;
-            if (tc < ns) o[tc] = vc;
-            if (td < ns) o[td] = vd;
+        } else {
+            for (int i = tid; i < V; i += nthr) {
+                const cpd z = B[tpos[i]];
+                float va = f2x_lo(z.x), vc = f2x_hi(z.x), vb = f2x_lo(z.y), vd = f2x_hi(z.y);
+                if (!SAME && xp.normalize) {
+                    const float4 c = Pc[i >> 3];
+                    const half4 f = Pf[i];
+                    const float2 fac = __half22float2(f.ac), fbd = __half22float2(f.bd);
+                    va += mu * (c.x + fac.x); vb += mu * (c.y + fbd.x); vc += mu * (c.z + fac.y); vd += mu * (c.w + fbd.y);
+                }
+                const int ta = t0 + i, tb = ta + V, tc = tb + V, td = tc + V;
+                if (ta < ns) o[ta] = va;
+                if (tb < ns) o[tb] = vb;
+                if (tc < ns) o[tc] = vc;
+                if (td < ns) o[td] = vd;
+            }
         }
         __syncthreads();
     }

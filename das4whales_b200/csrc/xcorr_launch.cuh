@@ -35,13 +35,15 @@ static int xcorr_launch(d4w_fft_plan* p, const float* x, int nx, int ns, int val
     xp.pl = p->pl; xp.tw = p->d_tw; xp.nb = p->n; xp.valid = valid; xp.ntpl = ntpl; xp.ns = ns;
     xp.normalize = dev_stats != nullptr ? 1 : 0;
     xp.nseg = (ns + valid - 1) / valid;
-    // dual-lane kernel (four segments per CTA, packed f32x2 butterflies): needs the fused plan shape; 2 CTAs per SM
-    const size_t smem_dual = (size_t)2 * p->n * 16 + (size_t)((valid + 7) / 8) * 16 + (size_t)valid * 8 + 16;
+    // dual-lane kernel (four segments per CTA, packed f32x2 butterflies): needs the fused plan shape; 2 CTAs per SM.
+    // Shared memory: S and B (16 B per sample each) and the mu-term prefix per group of 8 samples.
+    const size_t smem_dual = (size_t)2 * p->n * 16 + (size_t)((valid + 7) / 8) * 16 + 16;
     if (p->pfa) {
+        const size_t smem_pfa = smem_dual + (size_t)valid * 8;                   // + the fp16 in-group prefixes
         D4W_CUDA_TRY(cudaFuncSetAttribute(k_xcorr_pfa<SAME>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
-        if (smem_dual > 112 * 1024) return fail(D4W_ERR_UNSUPPORTED, std::string(fn) + ": shared memory");
+        if (smem_pfa > 112 * 1024) return fail(D4W_ERR_UNSUPPORTED, std::string(fn) + ": shared memory");
         dim3 gridp((xp.nseg + 3) / 4, nx);
-        k_xcorr_pfa<SAME><<<gridp, kPfaThreads, smem_dual, (cudaStream_t)stream>>>(xp, p->d_tpos, x, (const float2*)dev_tabs, dev_stats,
+        k_xcorr_pfa<SAME><<<gridp, kPfaThreads, smem_pfa, (cudaStream_t)stream>>>(xp, p->d_tpos, x, (const float2*)dev_tabs, dev_stats,
                                                                           dev_segpre, dev_mu_over_m, out, (size_t)nx * ns,
                                                                           dev_rowmax, lag0);
         D4W_CHECK_LAUNCH("k_xcorr_pfa");

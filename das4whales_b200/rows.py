@@ -94,9 +94,12 @@ def row_stats(x, seglen=0):
 # ------------------------------------------------------------------------------ matched filter
 def _pick_block(L, ns=0):
     """Overlap-save block length for templates of L taps.  2520 = 5 * 7 * 8 * 9: prime-factor blocks (no twiddles,
-    csrc/fft_pfa.cuh), the default up to 315 taps (>= 87 % of each block valid); longer templates use Cooley-Tukey blocks of
-    2500 / 5000 samples (three float2 buffers of a block must fit one SM's shared memory, so 5000 is the largest block and
-    2500 taps the longest template one pass can take -- detect.shift_xcorr cuts longer ones into pieces)."""
+    csrc/fft_pfa.cuh), the default up to 315 taps (>= 87 % of each block valid); longer templates, and rows that would need
+    more than 512 segments of 2520-sample blocks, use Cooley-Tukey blocks of 5000 samples (three float2 buffers of a block
+    must fit one SM's shared memory, so 5000 is the largest block and 2500 taps the longest template one pass can take --
+    detect.shift_xcorr cuts longer ones into pieces).  Only 2520 and 5000 are ever returned: 1250 and 2500 take at most
+    156 / 312 taps, and their segments are shorter than those of 2520-sample blocks, so whenever 2520 is rejected for its
+    segment count they are too (the tests force them to reach k_xcorr_dual)."""
     def nseg(nb):
         return (ns + (nb - L)) // (nb - L + 1) if ns else 0
     if L <= 2520 // 8 and nseg(2520) <= 512:
@@ -122,14 +125,16 @@ def cross_correlogram(x, templates, normalize=True):
         nz = np.nonzero(t)[0]
         L = int(nz[-1]) + 1 if len(nz) else 1
         c = t[:L]
+        taps.append(c)
         if normalize:
+            # the padded template minus its mean: out[i] = (sum_{n<L} x~[i+n] c[n] - mu * sum_{j>=i} x~[j]) / m, and the
+            # suffix sum is minus the exclusive prefix because x~ sums to zero -- so the raw taps c plus (mu / m) * prefix
             m = float(np.max(np.abs(t)))              # detect.py:158: abs-max of the un-demeaned template
             mu = float(np.sum(c) / len(t))            # mean of the PADDED template
-            taps.append(c - mu)                       # taps of (template - mean) inside the support ...
-            mus.append(mu / m)                        # ... and -mu/m outside it (handled as a prefix-sum term)
+            mus.append(mu / m)
             ms.append(m)
         else:
-            taps.append(c); mus.append(0.0); ms.append(1.0)
+            mus.append(0.0); ms.append(1.0)
     Lmax = max(len(c) for c in taps)
     nb = _pick_block(Lmax, ns)
     valid = nb - Lmax + 1

@@ -94,7 +94,8 @@ def test_script_notes_match_scipy(dw, ns):
 @pytest.mark.parametrize("L", [137, 400, 401, 2500])
 @pytest.mark.parametrize("ns", [1200, 12000, 12001])
 def test_long_and_odd_templates_match_scipy(dw, L, ns):
-    """400 / 401 taps run on 1 250- or 2 500-sample Cooley-Tukey blocks, 2 500 taps on 5 000-sample blocks."""
+    """137 taps run on 2 520-sample prime-factor blocks; 400, 401 and 2 500 taps on 5 000-sample Cooley-Tukey blocks
+    (rows._pick_block).  test_xcorr_routes_gpu.py forces the other block lengths."""
     x = _rows(24, ns, L + ns)
     c = _tpl(L, L)
     _check(dw.detect.compute_cross_correlogram_same(x, c), same_ref(x, c))
