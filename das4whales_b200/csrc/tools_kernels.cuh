@@ -1,0 +1,185 @@
+// tools_kernels.cuh -- __host__ __device__ bodies of the Gaussian-blurred f-k fan (tools.fk_filt_chunk, tools.py:27-49, and
+// the legacy dsp.fk_filt, dsp.py:883-953) and of the per-row moments / linear detrend (scipy.signal.detrend(type='linear'),
+// tools._energy_TimeDomain_chunk).  The same bodies run on the GPU (d4w_tools.cu) and on the host (tests/host_emul).
+//
+// The fan before the blur, G = g + fliplr(g) - g2 - fliplr(g2) with g = [f < k c_min and f < -k c_min], is a sum of four
+// signed index intervals along every row: f_j = (j - ns/2) fval increases with j, so [f_j < k c and f_j < -k c] holds on a
+// prefix [0, J) of the row, and its np.fliplr on the suffix [ns - J, ns).  The axis-1 blur of G is therefore exact from the
+// cumulative Gaussian weights (no input read), and only the axis-0 blur needs the 2r + 1 taps.  scipy.ndimage blurs axis 0
+// first; the two passes commute, so only the rounding of the float64 sums differs.
+#pragma once
+#include <cmath>
+#include <cstring>
+
+namespace d4w {
+
+constexpr int kFanTJ = 32;                      // columns per CTA (one per lane)
+constexpr int kFanU = 8;                        // consecutive output rows per thread
+constexpr int kFanG = 8;                        // row groups (warps) per CTA
+constexpr int kFanRT = kFanU * kFanG;           // output rows per CTA
+constexpr int kFanThreads = kFanTJ * kFanG;
+
+// scipy.ndimage.gaussian_filter's default truncate = 4: radius = int(4 sigma + 0.5)
+__host__ __device__ inline int fan_radius(double sigma) { return (int)(4.0 * sigma + 0.5); }
+// taps read by the sliding accumulation: 2r + U rounded up to U (the weights beyond 2r are zero)
+__host__ __device__ inline int fan_steps(int r) { return (2 * r + kFanU + kFanU - 1) / kFanU * kFanU; }
+__host__ __device__ inline int fan_tile_rows(int r) { return kFanRT + 2 * r + kFanU; }
+__host__ __device__ inline size_t fan_smem_bytes(int r) {
+    return sizeof(double) * ((size_t)fan_steps(r) + (size_t)(2 * r + 2) + (size_t)fan_tile_rows(r) * kFanTJ);
+}
+// workspace: min / max keys, weights w[2r + 1], cumulative weights cw[2r + 2], the row prefixes J[nx][2]
+__host__ __device__ inline size_t fan_ws_bytes(int nx, int r) {
+    return 16 + sizeof(double) * ((size_t)(2 * r + 1) + (size_t)(2 * r + 2)) + sizeof(int) * 2 * (size_t)nx;
+}
+
+struct FanParams {
+    int nx, ns, r;
+    double kval, fval, c_min, c_max;
+    const double* w;    // [2r + 1]
+    const double* cw;   // [2r + 2], cw[m] = w[0] + ... + w[m - 1]
+    const int* J;       // [nx][2]
+};
+
+// scipy.ndimage 'reflect' (d c b a | a b c d | d c b a), repeated for any p: the extension has period 2n
+__host__ __device__ inline int reflect_index(long long p, int n) {
+    const long long two = 2LL * n;
+    long long m = p % two;
+    if (m < 0) m += two;
+    return (int)(m < n ? m : two - 1 - m);
+}
+
+// number of columns j with f_j < prod and f_j < -prod, f_j = (j - ns/2) * fval as numpy.fft.fftfreq forms it; fval > 0 makes
+// the set a prefix, found by bisection on the reference's own comparisons
+__host__ __device__ inline int fan_prefix(int ns, double fval, double prod) {
+    int lo = 0, hi = ns;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        const double f = (double)(mid - ns / 2) * fval;
+        if (f < prod && f < -prod) lo = mid + 1; else hi = mid;
+    }
+    return lo;
+}
+
+// row i: k_i = (i - nx/2) * kval; J[i] = the prefixes of g (c_min) and g2 (c_max), products in the reference's order (kk * c)
+__host__ __device__ inline void body_fan_row(int nx, int ns, double kval, double fval, double c_min, double c_max, int* J, int i) {
+    const double k = (double)(i - nx / 2) * kval;
+    J[2 * i] = fan_prefix(ns, fval, k * c_min);
+    J[2 * i + 1] = fan_prefix(ns, fval, k * c_max);
+}
+
+// scipy.ndimage._gaussian_kernel1d(sigma, 0, r): exp(-0.5 / sigma^2 * x^2), x = -r..r, over its sum; and the running sums
+__host__ __device__ inline void fan_weights(double sigma, int r, double* w, double* cw) {
+    const double c = -0.5 / (sigma * sigma);
+    double s = 0.0;
+    for (int x = -r; x <= r; ++x) {
+        w[x + r] = exp(c * (double)((long long)x * x));
+        s += w[x + r];
+    }
+    cw[0] = 0.0;
+    for (int m = 0; m <= 2 * r; ++m) {
+        w[m] /= s;
+        cw[m + 1] = cw[m] + w[m];
+    }
+}
+
+__host__ __device__ inline long long floor_div(long long a, long long b) {
+    const long long q = a / b;
+    return (a % b != 0 && ((a < 0) != (b < 0))) ? q - 1 : q;
+}
+
+// sum_{s = -r..r} w_s [reflect(j + s) in [a, b)]: every copy of [a, b) in the period-2n extension that meets the window
+// [j - r, j + r] adds a difference of cumulative weights
+__host__ __device__ inline double interval_blur(const double* cw, int r, int n, int a, int b, int j) {
+    if (a >= b) return 0.0;
+    const long long lo = (long long)j - r, hi = (long long)j + r + 1, two = 2LL * n;
+    double acc = 0.0;
+    for (long long q = floor_div(lo, two) - 1; q <= floor_div(hi - 1, two); ++q) {
+        const long long base = q * two;
+        const long long c0[2] = {base + a, base + two - b}, c1[2] = {base + b, base + two - a};
+        for (int h = 0; h < 2; ++h) {
+            const long long s = c0[h] > lo ? c0[h] : lo, e = c1[h] < hi ? c1[h] : hi;
+            if (s < e) acc += cw[e - j + r] - cw[s - j + r];
+        }
+    }
+    return acc;
+}
+
+// the axis-1 blur of G at row i (already reflected into [0, nx)), column j.  [0, J1) - [0, J2) is the signed interval between
+// the two prefixes (likewise the suffixes), so a row where g = g2 blurs to exactly 0, as scipy's does
+__host__ __device__ inline double fan_row_blur(const FanParams& p, const double* cw, int i, int j) {
+    const int j1 = p.J[2 * i], j2 = p.J[2 * i + 1], n = p.ns;
+    const int lo = j1 < j2 ? j1 : j2, hi = j1 < j2 ? j2 : j1;
+    const double v = interval_blur(cw, p.r, n, lo, hi, j) + interval_blur(cw, p.r, n, n - hi, n - lo, j);
+    return j1 < j2 ? -v : v;
+}
+
+// shared copies of the weights, zero-padded to wz[fan_steps(r)], and of cw[2r + 2]
+__host__ __device__ inline void body_fan_weights(const FanParams& p, double* wz, double* cw, int tid, int nthr) {
+    const int S = fan_steps(p.r);
+    for (int s = tid; s < S; s += nthr) wz[s] = s <= 2 * p.r ? p.w[s] : 0.0;
+    for (int m = tid; m < 2 * p.r + 2; m += nthr) cw[m] = p.cw[m];
+}
+// CTA (i0, j0): the shared tile H[tr][c] = axis-1 blur at row reflect(i0 - r + tr), column j0 + c
+__host__ __device__ inline void body_fan_fill_tile(const FanParams& p, int i0, int j0, const double* cw, double* H, int tid, int nthr) {
+    const int rows = fan_tile_rows(p.r);
+    for (int idx = tid; idx < rows * kFanTJ; idx += nthr) {
+        const int tr = idx / kFanTJ, c = idx % kFanTJ, j = j0 + c;
+        H[idx] = j < p.ns ? fan_row_blur(p, cw, reflect_index((long long)i0 - p.r + tr, p.nx), j) : 0.0;
+    }
+}
+
+// thread (g, lane): acc[u] = sum_{t = 0..2r} w[t] H[g U + u + t][lane], the axis-0 blur at row i0 + g U + u.  Each tile value
+// is read once and feeds U accumulators; the U weights in flight sit in a register ring (static indices after unrolling).
+__host__ __device__ inline void body_fan_taps(const FanParams& p, const double* wz, const double* H, int g, int lane, double* acc) {
+    double wr[kFanU];
+#pragma unroll
+    for (int u = 0; u < kFanU; ++u) { acc[u] = 0.0; wr[u] = 0.0; }
+    const int S = fan_steps(p.r);
+    const double* col = H + (size_t)g * kFanU * kFanTJ + lane;
+    for (int s0 = 0; s0 < S; s0 += kFanU) {
+#pragma unroll
+        for (int v = 0; v < kFanU; ++v) {
+            const double d = col[(size_t)(s0 + v) * kFanTJ];
+            wr[v] = wz[s0 + v];
+#pragma unroll
+            for (int u = 0; u < kFanU; ++u) acc[u] = fma(wr[(v - u + kFanU) % kFanU], d, acc[u]);
+        }
+    }
+}
+
+// order-preserving map of a double onto unsigned 64-bit keys (for atomicMin / atomicMax); NaN is never produced here
+__host__ __device__ inline unsigned long long fan_key(double x) {
+    unsigned long long b;
+    memcpy(&b, &x, 8);
+    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+__host__ __device__ inline double fan_unkey(unsigned long long k) {
+    const unsigned long long b = (k >> 63) ? (k & 0x7fffffffffffffffull) : ~k;
+    double x;
+    memcpy(&x, &b, 8);
+    return x;
+}
+
+// ---- per-row moments over time chunks, and the linear detrend --------------------------------------------------------------
+// partial sums of one thread over the chunk [c0, c0 + len) of a row: s[0] = sum x, s[1] = sum t x (t from 0 at the chunk
+// start), s[2] = sum x^2, in float64
+__host__ __device__ inline void body_moments(const float* row, int len, int tid, int nthr, double* s) {
+    double a = 0.0, b = 0.0, q = 0.0;
+    for (int t = tid; t < len; t += nthr) {
+        const double v = row[t];
+        a += v;
+        b = fma((double)t, v, b);
+        q = fma(v, v, q);
+    }
+    s[0] = a; s[1] = b; s[2] = q;
+}
+
+// y = x - (least-squares line of the n samples): mean + slope (t - (n - 1)/2), slope = sum (t - (n-1)/2) x / (n (n^2 - 1) / 12)
+__host__ __device__ inline float detrend_sample(float x, int t, int n, const double* m) {
+    const double mean = m[0] / n, h = 0.5 * (n - 1);
+    const double den = (double)n * ((double)n * n - 1.0) / 12.0;
+    const double slope = n > 1 ? (m[1] - h * m[0]) / den : 0.0;
+    return (float)((double)x - mean - slope * ((double)t - h));
+}
+
+}  // namespace d4w

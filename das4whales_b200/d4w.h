@@ -335,6 +335,24 @@ int d4w_radon(const float* dev_img, int h, int w, int n, int pad_r, int pad_c, c
 int d4w_bilateral(const float* dev_in, int h, int w, int is_8u, int radius, double sigma_color, double sigma_space,
                   void* dev_workspace, float* dev_out, void* stream);
 int d4w_grad_oriented(const float* dev_in, int h, int w, int dft, int dfx, float* dev_out, void* stream);
+
+/* ---- the tools module (das4whales/tools.py:8-157) and the legacy dsp.fk_filt (dsp.py:883-953).
+ *  d4w_fan_blur: the Gaussian-blurred speed fan, float32 [nx][ns] in the reference's shifted layout: with
+ *      f_j = (j - ns/2) fval, k_i = (i - nx/2) kval (numpy.fft.fftfreq's products), g = [f < k c_min and f < -k c_min],
+ *      g2 the same with c_max, G = g + fliplr(g) - g2 - fliplr(g2), blurred as scipy.ndimage.gaussian_filter(G, sigma)
+ *      (truncate 4, mode 'reflect', repeated for a radius beyond an axis) in float64 and normalised as
+ *      (G - min) / (max - min): NaN everywhere when max == min, as NumPy's 0 / 0.  fval > 0.  The radius int(4 sigma + 0.5)
+ *      must leave the shared tile within 227 KB (sigma up to about 100).  dev_workspace: d4w_fan_blur_workspace_bytes.
+ *  d4w_row_moments: sum x, sum t x and sum x^2 in float64 of every time chunk of every row: row r is the n samples at
+ *      dev_x + r * ld, chunk c its samples [c chunk, min((c + 1) chunk, n)), t counted from the chunk start.
+ *      dev_out: double [nrows][ceil(n / chunk)][3].
+ *  d4w_detrend_linear: scipy.signal.detrend(type='linear', axis=-1) of the same rows (moments of chunk = n from
+ *      d4w_row_moments), written contiguously: dev_y float32 [nrows][n].  nrows <= 65 535. */
+size_t d4w_fan_blur_workspace_bytes(int nx, double sigma);
+int d4w_fan_blur(float* dev_out, int nx, int ns, double kval, double fval, double c_min, double c_max, double sigma,
+                 void* dev_workspace, void* stream);
+int d4w_row_moments(const float* dev_x, size_t ld, int nrows, int n, int chunk, double* dev_out, void* stream);
+int d4w_detrend_linear(const float* dev_x, size_t ld, int nrows, int n, const double* dev_moments, float* dev_y, void* stream);
 /* D4W_CDEF_END */
 
 #ifdef __cplusplus

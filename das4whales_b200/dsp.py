@@ -175,18 +175,13 @@ def hybrid_ninf_gs_filter_design(trace_shape, selected_channels, dx, fs, cs_min=
 
 def fk_filt(data, tint, fs, xint, dx, c_min, c_max):
     """Legacy one-call f-k filter: Gaussian-blurred boolean fan built and applied in one go
-    (reference: dsp.py:883-953).  The fan is built on the host, the 2-D filtering runs on the GPU."""
-    from scipy import ndimage
-    shape = tuple(data.shape)
-    f = np.fft.fftshift(np.fft.fftfreq(shape[1], d=tint / fs))
-    k = np.fft.fftshift(np.fft.fftfreq(shape[0], d=xint * dx))
-    ff, kk = np.meshgrid(f, k)
-    g = 1.0 * ((ff < kk * c_min) & (ff < -kk * c_min))
-    g2 = 1.0 * ((ff < kk * c_max) & (ff < -kk * c_max))
-    g = g + g[:, ::-1] - (g2 + g2[:, ::-1])
-    g = ndimage.gaussian_filter(g, 20)
-    g = (g - np.min(g)) / (np.max(g) - np.min(g))
-    return fk_filter_filt(data, _fk.FkMask.from_dense(g))
+    (reference: dsp.py:883-953).  The fan (sigma = 20) is designed on the GPU (rows.blurred_fan) and goes to the filter as
+    a device tensor: the [nx, ns] plane never exists on the host."""
+    nx, ns = (int(n) for n in data.shape)
+    # numpy.fft.fftfreq(n, d) steps 1 / (n * d), d = tint / fs and xint * dx (dsp.py:931-932)
+    kval, fval = 1.0 / (nx * (xint * dx)), 1.0 / (ns * (tint / fs))
+    dev = data.device.index if _is_tensor(data) and data.is_cuda else None
+    return fk_filter_filt(data, _rows.blurred_fan(nx, ns, kval, fval, c_min, c_max, 20, device=dev))
 
 
 def _display_mask(mask, freq, knum):

@@ -600,3 +600,64 @@ def raw2strain(raw2d, scale_factor):
         _lib.check(_lib.lib().d4w_raw2strain(_lib.ffi.cast("void*", raw2d.data_ptr()), 1 if raw2d.dtype == torch.int32 else 0,
                                              rows_, n, float(scale_factor), _lib.ptr(out, "float*"), _lib.stream_ptr()), "raw2strain")
     return out
+
+
+# ------------------------------------------------------------------------------ moments, linear detrend, blurred f-k fan
+def _check_rows_view(x):
+    """float32 CUDA [rows, n] tensor whose samples are contiguous along time (a block view of a larger matrix is fine)"""
+    torch = _torch()
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.ndim == 2):
+        raise ValueError("expected a float32 CUDA tensor [channels, samples]")
+    if x.shape[1] > 1 and x.stride(1) != 1 or x.stride(0) < x.shape[1]:
+        raise ValueError("expected rows with unit time stride (a row block of a C-ordered matrix)")
+    return x.device.index
+
+
+def row_moments(x, chunk=None):
+    """[rows, ceil(n / chunk), 3] float64 CUDA: sum x, sum t x (t counted from the chunk start) and sum x^2 of every time
+    chunk of every row of x (chunk=None: the whole row), d4w_row_moments."""
+    torch = _torch()
+    dev = _check_rows_view(x)
+    rows_, n = x.shape
+    chunk = n if chunk is None else int(chunk)
+    out = torch.empty((rows_, -(-n // chunk), 3), dtype=torch.float64, device=x.device)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().d4w_row_moments(_lib.ptr(x, "float*"), max(x.stride(0), n), rows_, n, chunk,
+                                              _lib.ptr(out, "double*"), _lib.stream_ptr()), "row_moments")
+    return out
+
+
+def detrend_linear(x, out=None):
+    """scipy.signal.detrend(x, type='linear', axis=-1) of every row, moments in float64: a contiguous float32 [rows, n] copy
+    (x may be a block view of a larger matrix, read in the same pass)."""
+    torch = _torch()
+    dev = _check_rows_view(x)
+    rows_, n = x.shape
+    mom = row_moments(x)
+    if out is None:
+        out = torch.empty((rows_, n), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(dev):
+        for r0 in range(0, rows_, 65535):
+            r1 = min(rows_, r0 + 65535)
+            _lib.check(_lib.lib().d4w_detrend_linear(_lib.ptr(x[r0:r1], "float*"), max(x.stride(0), n), r1 - r0, n,
+                                                     _lib.ptr(mom[r0:r1], "double*"), _lib.ptr(out[r0:r1], "float*"),
+                                                     _lib.stream_ptr()), "detrend_linear")
+    return out
+
+
+def blurred_fan(nx, ns, kval, fval, c_min, c_max, sigma, device=None):
+    """The normalised Gaussian-blurred speed fan of dsp.fk_filt (sigma 20) and tools.fk_filt_chunk (sigma 40) as a float32
+    CUDA [nx, ns] tensor in the reference's shifted layout, designed on the device (d4w_fan_blur); kval / fval are
+    numpy.fft.fftfreq's steps.  NaN everywhere when the blurred fan is constant, as the reference's 0 / 0."""
+    torch = _torch()
+    dev = torch.cuda.current_device() if device is None else int(device)
+    L = _lib.lib()
+    ws_bytes = L.d4w_fan_blur_workspace_bytes(int(nx), float(sigma))
+    if ws_bytes == 0:
+        raise ValueError(f"blurred_fan: sigma = {sigma} must be > 0 and nx = {nx} >= 1")
+    out = torch.empty((int(nx), int(ns)), dtype=torch.float32, device=f"cuda:{dev}")
+    ws = torch.empty(int(ws_bytes), dtype=torch.uint8, device=f"cuda:{dev}")
+    with torch.cuda.device(dev):
+        _lib.check(L.d4w_fan_blur(_lib.ptr(out, "float*"), int(nx), int(ns), float(kval), float(fval), float(c_min), float(c_max),
+                                  float(sigma), _lib.ptr(ws), _lib.stream_ptr()), "blurred_fan")
+    return out
