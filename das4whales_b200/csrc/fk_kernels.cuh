@@ -625,8 +625,10 @@ __host__ __device__ inline void body_row_mid_dual(const RowParams& rp, float2* _
 //   level B: X2-point FFT over c2 in shared memory, wide coalesced tiles, several CTAs per SM
 // Real input => only planes k1 = 0..X1/2 of the intermediate V are stored (Hermitian in k1), and the
 // outputs of plane X1-k1 are conj(P_{k1}[X2-1-k2]) of the same level-B transform, so each kept
-// wavenumber row is produced exactly once.  V[plane][c2][sample pair] holds 16-byte elements
-// {re_t, re_t+1, im_t, im_t+1}.  Forward: A then B (pruned rows out); inverse: B then A.
+// wavenumber row is produced exactly once.  V[plane][c2][position] holds 16-byte elements
+// {re_t, re_t+1, im_t, im_t+1}, one per sample pair; chunk pair p sits at position vpos(p, vhp) (below), so that
+// level A, whose thread owns the pairs 2q and 2q + 1, accesses whole 32-byte sectors.  Forward: A then B (pruned rows out);
+// inverse: B then A.
 struct Col2Params {
     FftPlan plb;             // X2-point plan (dual lanes)
     const float2* twb;       // W_X2^j
@@ -637,6 +639,14 @@ struct Col2Params {
     // intermediate V holds just this chunk (row stride vhp pairs) so that it stays resident in L2 between the two
     int vhp, tpb, tpn;
 };
+
+// Position of chunk pair p inside a row of V (vhp pairs): inside each group of 8 pairs (128 bytes) the even pairs fill
+// the first 64 bytes and the odd pairs the second.  A warp of level-A threads (consecutive quads q, pairs 2q and 2q + 1)
+// then stores or loads 64-byte runs of whole sectors, where the natural order put its 16-byte accesses 32 bytes apart
+// (half sectors, every sector touched by both instructions); level B's 8-pair tile stays one 128-byte line per row.
+// Pairs past the last whole group (vhp not a multiple of 8) keep their natural position.  The map depends on the pair
+// and the plan's row length only, so a ragged last chunk (fewer pairs than vhp) needs nothing of its own.
+D4W_HD int vpos(int p, int vhp) { return p < (vhp & ~7) ? (p & ~7) | ((p >> 1) & 3) | ((p & 1) << 2) : p; }
 
 // ---- global-memory access with an L2 eviction policy (pipelined level A/B kernel) -------------------------------
 // `keep` (evict_last) is used for the chunk ring of the intermediate V, which must survive in L2 from its producer
@@ -696,6 +706,7 @@ __host__ __device__ inline void body_colA_fwd(const Col2Params& cp, const float*
     const int ns = cp.ns, x2 = cp.x2;
     const size_t hp = (size_t)cp.vhp;
     const size_t tg = 4 * (size_t)(tpb / 2 + t4);      // first of this thread's four samples in the record
+    const int pa = vpos(2 * t4, cp.vhp), pd = vpos(2 * t4 + 1, cp.vhp) - pa;     // V positions of this thread's pairs
     cpd v[X1];
     float2 twp[X1 / 2 + 1];                                          // W_nx^{c2 k1}, k1 = 0 .. X1/2, from one table read
     twiddle_powers<X1 / 2 + 1>(cp.twn[c2], twp);
@@ -722,8 +733,8 @@ __host__ __device__ inline void body_colA_fwd(const Col2Params& cp, const float*
         } else {
             fa = dmake(vmul(fa.x, half), vmul(fa.y, half)); fb = dmake(vmul(fb.x, half), vmul(fb.y, half));
         }
-        cpd* o = v2 + ((size_t)k1 * x2 + c2) * hp + 2 * t4;
-        stc<PIPE>(o, fa, pol.keep); stc<PIPE>(o + 1, fb, pol.keep);
+        cpd* o = v2 + ((size_t)k1 * x2 + c2) * hp + pa;
+        stc<PIPE>(o, fa, pol.keep); stc<PIPE>(o + pd, fb, pol.keep);
     });
 }
 template <int X1, bool PIPE = false>
@@ -732,13 +743,14 @@ __host__ __device__ inline void body_colA_inv(const Col2Params& cp, const cpd* _
     const int ns = cp.ns, x2 = cp.x2;
     const size_t hp = (size_t)cp.vhp;
     const size_t tg = 4 * (size_t)(tpb / 2 + t4);
+    const int pa = vpos(2 * t4, cp.vhp), pd = vpos(2 * t4 + 1, cp.vhp) - pa;
     cpd v[X1];
     float2 twp[X1 / 2 + 1];
     twiddle_powers<X1 / 2 + 1>(cp.twn[c2], twp);
     static_for<X1 / 2 + 1>([&](auto kc) {
         constexpr int k1 = decltype(kc)::value;
-        const cpd* in = v2 + ((size_t)k1 * x2 + c2) * hp + 2 * t4;
-        cpd fa = ldc<PIPE>(in, pol.keep), fb = ldc<PIPE>(in + 1, pol.keep);
+        const cpd* in = v2 + ((size_t)k1 * x2 + c2) * hp + pa;
+        cpd fa = ldc<PIPE>(in, pol.keep), fb = ldc<PIPE>(in + pd, pol.keep);
         if (k1 > 0) { const float2 w = twp[k1]; fa = dmulc_s(fa, w); fb = dmulc_s(fb, w); }
         if (k1 == 0 || 2 * k1 == X1) {                       // self-conjugate in k1: real
             v[k1] = dmake(fa.x, fb.x);
@@ -765,7 +777,7 @@ __host__ __device__ inline void body_colB_fwd(const Col2Params& cp, const cpd* _
     const int sh = cp.np_shift;
     for (int i = tid; i < (x2 << sh); i += nthr) {
         const int c2 = i >> sh, j = i & (np - 1);
-        const cpd* src = v2 + ((size_t)plane * x2 + c2) * hp + tp0 + j;
+        const cpd* src = v2 + ((size_t)plane * x2 + c2) * hp + vpos(tp0 + j, hp);
 #ifdef __CUDA_ARCH__
         if (tp0 + j < tpn) cp_async16(smem + j * cp.fstride + c2, src); else smem[j * cp.fstride + c2] = zero;
 #else
@@ -812,7 +824,7 @@ __host__ __device__ inline void body_colB_inv(const Col2Params& cp, cpd* __restr
     fft_inverse_stages_dual(smem, cp.plb, cp.twb, np, cp.fstride, tid, nthr);
     for (int i = tid; i < (x2 << sh); i += nthr) {
         const int c2 = i >> sh, j = i & (np - 1);
-        if (tp0 + j < tpn) v2[((size_t)plane * x2 + c2) * hp + tp0 + j] = smem[j * cp.fstride + c2];
+        if (tp0 + j < tpn) v2[((size_t)plane * x2 + c2) * hp + vpos(tp0 + j, hp)] = smem[j * cp.fstride + c2];
     }
 }
 
@@ -833,7 +845,7 @@ __host__ __device__ inline void body_colB_fwd_fused(const Col2Params& cp, const 
         const int n = it >> sh, j = it & (np - 1);
         const bool ok = tp0 + j < tpn;
         cpd v[RA];
-        const cpd* src = v2 + ((size_t)plane * x2 + n) * hp + tp0 + j;
+        const cpd* src = v2 + ((size_t)plane * x2 + n) * hp + vpos(tp0 + j, hp);
         static_for<RA>([&](auto qc) { constexpr int q = decltype(qc)::value; v[q] = ok ? ldc<PIPE>(src + (size_t)(RB * q) * hp, pol.keep) : zero; });
         DFTD<RA, false>::run(v);
         apply_stage_twiddles<RA, false, true>(v, cp.twb[n]);
@@ -895,7 +907,7 @@ __host__ __device__ inline void body_colB_inv_fused(const Col2Params& cp, cpd* _
         static_for<RA>([&](auto mc) { constexpr int m = decltype(mc)::value; v[m] = src[RB * m]; });
         apply_stage_twiddles<RA, true, false>(v, cp.twb[n]);
         DFTD<RA, true>::run(v);
-        cpd* dst = v2 + ((size_t)plane * x2 + n) * hp + tp0 + j;
+        cpd* dst = v2 + ((size_t)plane * x2 + n) * hp + vpos(tp0 + j, hp);
         static_for<RA>([&](auto qc) { constexpr int q = decltype(qc)::value; stc<PIPE>(dst + (size_t)(RB * q) * hp, v[outpos<RA>(q)], pol.keep); });
     }
 }
@@ -920,7 +932,7 @@ __host__ __device__ inline void body_colB3_fwd(const Col2Params& cp, const cpd* 
         const int n = it >> sh, j = it & (np - 1);
         const bool ok = tp0 + j < tpn;
         cpd v[R0];
-        const cpd* src = v2 + ((size_t)plane * X2 + n) * hp + tp0 + j;
+        const cpd* src = v2 + ((size_t)plane * X2 + n) * hp + vpos(tp0 + j, hp);
         static_for<R0>([&](auto qc) { constexpr int q = decltype(qc)::value; v[q] = ok ? ldc<PIPE>(src + (size_t)(L0 * q) * hp, pol.keep) : zero; });
         DFTD<R0, false>::run(v);
         apply_stage_twiddles<R0, false, true>(v, cp.twb[n]);                       // W_X2^{n m}
@@ -1009,7 +1021,7 @@ __host__ __device__ inline void body_colB3_inv(const Col2Params& cp, cpd* __rest
         static_for<R0>([&](auto mc) { constexpr int m = decltype(mc)::value; v[m] = src[L0 * m]; });
         apply_stage_twiddles<R0, true, false>(v, cp.twb[n]);
         DFTD<R0, true>::run(v);
-        cpd* dst = v2 + ((size_t)plane * X2 + n) * hp + tp0 + j;
+        cpd* dst = v2 + ((size_t)plane * X2 + n) * hp + vpos(tp0 + j, hp);
         static_for<R0>([&](auto qc) { constexpr int q = decltype(qc)::value; stc<PIPE>(dst + (size_t)(L0 * q) * hp, v[outpos<R0>(q)], pol.keep); });
     }
 }

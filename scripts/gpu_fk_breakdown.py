@@ -6,7 +6,12 @@ Prints the card (name, power limit, SM clock), then for each of the five passes 
 (CUDA events, each pass launched alone), the HBM bytes the plan must move in it (FkFilter.traffic_bytes) and the rate
 that gives, the median time of a whole filter call, and a torch.profiler table of every kernel the call launches (a
 separate run, so the timings above carry no tracing overhead).  With --out, the table and the numbers go to
-DIR/fk_breakdown.json."""
+DIR/fk_breakdown.json.
+
+For the two-level column passes P1 and P5 it also reports the L2 sector bytes the plan moves and the rate that gives:
+x (or y), the level-A/B intermediate V written by one level and read by the other, and the kept rows W.  Level A moves
+V in whole 32-byte sectors with the blocked position order of the kernels in this tree; --v-layout natural counts V's
+level-A side at the half-sector efficiency of the earlier order (for timing a build of an earlier commit)."""
 import argparse
 import json
 import os
@@ -31,11 +36,33 @@ def card():
         return f"nvidia-smi unavailable: {exc!r}"
 
 
+def two_level_shape(nx):
+    """(X1, X2) of the planner's two-level column split: X1 the largest of 25, 20, 16 dividing nx with 8 <= X2 <= 1024"""
+    for x1 in (25, 20, 16):
+        if nx % x1 == 0 and 8 <= nx // x1 <= 1024:
+            return x1, nx // x1
+    return None
+
+
+def col_l2_sector_bytes(nx, ns, rows_kept, v_layout):
+    """L2 sector bytes of one two-level column pass (P1 or P5), from the plan's shape.  Every access is a whole
+    32-byte sector except level A's V accesses in the natural order, where each 16-byte access fills half of one."""
+    x1, x2 = two_level_shape(nx)
+    planes = x1 // 2 + 1
+    xy = nx * ns * 4                                   # x in (P1) or y out (P5)
+    v = planes * x2 * (ns // 2) * 16                   # V: one 16-byte element per plane, c2 row and sample pair
+    w = rows_kept * ns * 8                             # kept wavenumber rows, complex64
+    v_a = v * (2 if v_layout == "natural" else 1)
+    return {"x_or_y": xy, "v_level_a": v_a, "v_level_b": v, "w": w, "total": xy + v_a + v + w}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--out")
+    ap.add_argument("--v-layout", choices=("blocked", "natural"), default="blocked",
+                    help="position order of V inside a chunk row in the build being timed")
     args = ap.parse_args()
     import torch
     import das4whales_b200 as dw
@@ -79,6 +106,11 @@ def main():
         res["passes"][n] = {"ms": round(m, 4), "spread_ms": round(max(pass_ms[i]) - min(pass_ms[i]), 4),
                             "share": round(m / sum(statistics.median(p) for p in pass_ms), 4),
                             "plan_bytes": traffic[n], "gbs": round(traffic[n] / (m * 1e-3) / 1e9, 1) if m > 0 else None}
+        if n in ("p1_col_fwd", "p5_col_inv") and flt.plan.col_scheme in (2, 3):
+            l2 = col_l2_sector_bytes(NX, NS, flt.rows_kept, args.v_layout)
+            res["passes"][n]["l2_sector_bytes"] = l2
+            res["passes"][n]["l2_sector_gbs"] = round(l2["total"] / (m * 1e-3) / 1e9, 1) if m > 0 else None
+    res["v_layout"] = args.v_layout
     # torch.profiler: every kernel of 3 filter calls, in a run of its own
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
