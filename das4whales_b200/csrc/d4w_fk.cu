@@ -533,8 +533,19 @@ static int launch_col2_pipe(const d4w_fk_plan* pl, const d4w_fk_mask* m, const f
     return D4W_OK;
 }
 
-// One pass on explicit buffers, arguments already checked.  w: the kept rows of m's support; v2: the two-level
-// intermediate (nullptr: the single-level column kernels); tab: P3's table for the `slot_count` rows at w; w3: P3's
+// The column kernels move whole rows of x and y with 16-byte accesses when ns % 4 == 0 (cp.async, TMA tiles, the two-level
+// kernels) and 8-byte ones when ns is even, so a matrix must start on that boundary.  Checked before any launch: a
+// misaligned base would otherwise fault inside a kernel.
+static int check_matrix_alignment(const float* p, int ns, const char* what) {
+    const uintptr_t align = ns % 4 == 0 ? 16 : ns % 2 == 0 ? 8 : sizeof(float);
+    if (p && (uintptr_t)p % align)
+        return fail(D4W_ERR_ARG, std::string(what) + " must be " + std::to_string(align) + "-byte aligned for " + std::to_string(ns) +
+                                     " samples per row");
+    return D4W_OK;
+}
+
+// One pass on explicit buffers, arguments already checked (x and y aligned as check_matrix_alignment requires).
+// w: the kept rows of m's support; v2: the two-level intermediate (nullptr: the single-level column kernels); tab: P3's table for the `slot_count` rows at w; w3: P3's
 // destination (nullptr: in place, the single-mask filter; otherwise a second kept-row block of the same layout).
 static int fk_run_pass(const d4w_fk_plan* pl, const d4w_fk_mask* m, const float* x, float* y, float2* w, cpd* v2,
                        const float* tab, float2* w3, const float* tap, int pass, int slot_count, cudaStream_t stream) {
@@ -554,7 +565,7 @@ static int fk_run_pass(const d4w_fk_plan* pl, const d4w_fk_mask* m, const float*
                 D4W_CHECK_LAUNCH("k_col_fwd_czt");
                 return D4W_OK;
             }
-            if (two && ((uintptr_t)x % 16 == 0)) {
+            if (two) {
                 if (pl->pipe.nchunks && m->d_need) return launch_col2_pipe<false>(pl, m, x, nullptr, v2, w, ldw, tap, stream);
                 for (int tpb = 0; tpb < pl->ns / 2; tpb += pl->col2.vhp) {        // time chunks: V stays in L2 from A to B
                     Col2Params c2 = pl->col2;
@@ -573,7 +584,7 @@ static int fk_run_pass(const d4w_fk_plan* pl, const d4w_fk_mask* m, const float*
                 }
                 return D4W_OK;
             }
-            if (pl->col.tma && ((uintptr_t)x % 16 == 0)) {
+            if (pl->col.tma) {
                 CUtensorMap tm;
                 if (make_tile_map(&tm, x, pl->nx, pl->ns)) {
                     const int grid = std::min(ntiles, pl->num_sms);
@@ -639,7 +650,7 @@ static int fk_run_pass(const d4w_fk_plan* pl, const d4w_fk_mask* m, const float*
                 D4W_CHECK_LAUNCH("k_col_inv_czt");
                 return D4W_OK;
             }
-            if (two && ((uintptr_t)y % 16 == 0)) {
+            if (two) {
                 if (pl->pipe.nchunks && m->d_need) return launch_col2_pipe<true>(pl, m, nullptr, y, v2, w, ldw, nullptr, stream);
                 for (int tpb = 0; tpb < pl->ns / 2; tpb += pl->col2.vhp) {
                     Col2Params c2 = pl->col2;
@@ -658,7 +669,7 @@ static int fk_run_pass(const d4w_fk_plan* pl, const d4w_fk_mask* m, const float*
                 }
                 return D4W_OK;
             }
-            if (pl->col.tma && ((uintptr_t)y % 16 == 0)) {
+            if (pl->col.tma) {
                 CUtensorMap tm;
                 if (make_tile_map(&tm, y, pl->nx, pl->ns)) {
                     const int grid = std::min(ntiles, pl->num_sms);
@@ -719,6 +730,8 @@ extern "C" int d4w_fk_apply_pass_ex(d4w_fk_plan* pl, d4w_fk_mask* m, const float
         if (pl->ns != mp->ns) return fail(D4W_ERR_ARG, "d4w_fk_apply: time passes need the mask's full time axis");
         if (slot_begin < 0 || slot_count < 0 || slot_begin + slot_count > m->nact) return fail(D4W_ERR_ARG, "d4w_fk_apply: bad slot range");
     }
+    if (pass == 1 && check_matrix_alignment(x, pl->ns, "d4w_fk_apply: input") != D4W_OK) return D4W_ERR_ARG;
+    if (pass == 5 && check_matrix_alignment(y, pl->ns, "d4w_fk_apply: output") != D4W_OK) return D4W_ERR_ARG;
     const float* tap = taper ? mp->d_taper + t_offset : nullptr;
     cpd* v2 = use_two_level(pl, m, ws) ? reinterpret_cast<cpd*>(reinterpret_cast<char*>(ws) + kept_rows_bytes(pl, m->nact)) : nullptr;
     return fk_run_pass(pl, m, x, y, (float2*)ws, v2, m->d_table + (size_t)slot_begin * pl->ns, nullptr, tap, pass, slot_count,
@@ -734,6 +747,8 @@ extern "C" int d4w_fk_apply_pass(d4w_fk_plan* pl, d4w_fk_mask* m, const float* x
 
 extern "C" int d4w_fk_apply(d4w_fk_plan* pl, d4w_fk_mask* m, const float* x, float* y, void* ws, int taper,
                             void* stream) {
+    if (pl && (check_matrix_alignment(x, pl->ns, "d4w_fk_apply: input") != D4W_OK ||
+               check_matrix_alignment(y, pl->ns, "d4w_fk_apply: output") != D4W_OK)) return D4W_ERR_ARG;   // before P1 runs
     for (int pass = 1; pass <= 5; ++pass) {
         int rc = d4w_fk_apply_pass(pl, m, x, y, ws, taper, pass, stream);
         if (rc != D4W_OK) return rc;
@@ -848,11 +863,13 @@ extern "C" int d4w_fk_bank_apply_pass(d4w_fk_plan* pl, d4w_fk_bank* b, const flo
     const size_t bytes = (size_t)pl->nx * pl->ns * sizeof(float);
     for (int i = 0; i < nm; ++i) {
         if (!ys[i]) return fail(D4W_ERR_ARG, "d4w_fk_bank_apply: null output " + std::to_string(i));
+        if (check_matrix_alignment(ys[i], pl->ns, ("d4w_fk_bank_apply: output " + std::to_string(i)).c_str()) != D4W_OK) return D4W_ERR_ARG;
         for (int j = 0; j < i; ++j) {
             const char *a = (const char*)ys[i], *c = (const char*)ys[j];
             if (a < c + bytes && c < a + bytes) return fail(D4W_ERR_ARG, "d4w_fk_bank_apply: outputs " + std::to_string(j) + " and " + std::to_string(i) + " overlap");
         }
     }
+    if (pass == 1 && check_matrix_alignment(x, pl->ns, "d4w_fk_bank_apply: input") != D4W_OK) return D4W_ERR_ARG;
     DeviceGuard guard(pl->device);
     const d4w_fk_mask* sup = b->sup;
     const int nu = sup->nact;

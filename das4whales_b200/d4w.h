@@ -95,7 +95,9 @@ int d4w_fk_mask_materialize(const d4w_fk_mask* mask, double* dev_out, void* stre
 size_t d4w_fk_workspace_bytes(const d4w_fk_plan* plan, const d4w_fk_mask* mask);
 /* y = real(ifft2(ifftshift(fftshift(fft2(x)) * M))) with optional Tukey(alpha=0.03) taper
  * applied to x first (taper != 0; x itself is not modified).  x, y: float32 [nx x ns],
- * C order, device memory; y may alias x. */
+ * C order, device memory; y may alias x.  x and y must be 16-byte aligned when ns % 4 == 0
+ * and 8-byte aligned when ns is even, else D4W_ERR_ARG before any launch (the same holds for
+ * the pass-wise calls below and for the matrices of a mask bank). */
 int d4w_fk_apply(d4w_fk_plan* plan, d4w_fk_mask* mask, const float* dev_x, float* dev_y,
                  void* dev_workspace, int taper, void* stream);
 /* the five passes, separately (bench / profiling): pass = 1..5 */

@@ -44,6 +44,7 @@ class _Plan:
         self.t1, self.t2, self.tile, self.col_stages, self.row_stages = info[0], info[1], info[2], info[3], info[4]
         # column transform: 0 single-level, 1 single-level TMA, 2 two-level, 3 pipelined two-level, 4 chirp-z single-level
         self.col_scheme = int(info[7])
+        self.col_threads = int(info[5])      # block size of the single-level column kernels
         self.workspace = None
 
     def get_workspace(self, nbytes):
@@ -279,6 +280,13 @@ def device_mask_for(mask, plan, eps=0.0):
     return holder.dm
 
 
+def _misaligned(t, ns):
+    """True when t does not start on the boundary d4w_fk_apply needs for rows of ns samples (16 bytes when ns % 4 == 0,
+    8 when ns is even): a contiguous view that starts inside its allocation, such as buf[1:].view(nx, ns)."""
+    align = 16 if ns % 4 == 0 else 8 if ns % 2 == 0 else 4
+    return t.data_ptr() % align != 0
+
+
 class FkFilter:
     """Reusable f-k filter for one matrix shape: plan + mask table + workspace on one GPU.
 
@@ -307,13 +315,17 @@ class FkFilter:
             raise ValueError("FkFilter expects a contiguous float32 CUDA tensor")
         if tuple(x.shape) != (self.plan.nx, self.plan.ns):
             raise ValueError(f"FkFilter built for {(self.plan.nx, self.plan.ns)}, got {tuple(x.shape)}")
-        if out is None:
-            out = torch.empty_like(x)
+        ns = self.plan.ns
+        xin = x.clone() if _misaligned(x, ns) else x          # a misaligned matrix goes through an aligned copy
+        y = torch.empty_like(x) if out is None or _misaligned(out, ns) else out
         L = _lib.lib()
         with torch.cuda.device(self.device):
-            _lib.check(L.d4w_fk_apply(self.plan.ptr, self.dm.ptr, _lib.ptr(x, "float*"), _lib.ptr(out, "float*"),
+            _lib.check(L.d4w_fk_apply(self.plan.ptr, self.dm.ptr, _lib.ptr(xin, "float*"), _lib.ptr(y, "float*"),
                                       _lib.ptr(self._ws()), int(bool(tapering)), _lib.stream_ptr()), "fk_filter_filt")
-        return out
+        if out is not None and y is not out:
+            out.copy_(y)
+            return out
+        return y
 
     def run_pass(self, i, x, out, tapering=False):
         """Launch pass i (1..5) alone -- profiling / per-kernel timing."""
@@ -400,11 +412,24 @@ class FkFilterBank:
 
     def __call__(self, x, outs=None, tapering=False):
         """Filter x with every mask; returns the list of outputs.  One of `outs` may be x itself; no two may overlap."""
-        outs, ys = self._outs(x, outs)
+        outs, _ = self._outs(x, outs)
+        nbytes = x.numel() * 4
+        for i, o in enumerate(outs):          # checked on the caller's outputs, before any is swapped for a temporary
+            for j in range(i):
+                a, c = o.data_ptr(), outs[j].data_ptr()
+                if a < c + nbytes and c < a + nbytes:
+                    raise ValueError(f"FkFilterBank outputs {j} and {i} overlap")
+        ns = self.plan.ns
+        xin = x.clone() if _misaligned(x, ns) else x          # misaligned matrices go through aligned copies
+        run = [_torch().empty_like(o) if _misaligned(o, ns) else o for o in outs]
+        ys = _lib.ffi.new("float*[]", [_lib.ptr(o, "float*") for o in run])
         L = _lib.lib()
         with _torch().cuda.device(self.device):
-            _lib.check(L.d4w_fk_bank_apply(self.plan.ptr, self.ptr, _lib.ptr(x, "float*"), ys, _lib.ptr(self._ws()),
+            _lib.check(L.d4w_fk_bank_apply(self.plan.ptr, self.ptr, _lib.ptr(xin, "float*"), ys, _lib.ptr(self._ws()),
                                            int(bool(tapering)), _lib.stream_ptr()), "fk bank")
+        for o, r in zip(outs, run):
+            if r is not o:
+                o.copy_(r)
         return outs
 
     def run_pass(self, i, x, outs, tapering=False, mask=0):

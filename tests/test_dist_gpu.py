@@ -39,7 +39,7 @@ def _mask(dw, kind, nx, ns):
     (10000, 4800, 2, "fan", True, 1),        # 25 x 400: the pipelined kernels of the headline configuration, on 2400-sample slabs
     (10000, 4800, 4, "hybrid", False, 1),    # nothing pruned, 4 ranks, uneven row split (5001 rows)
     (600, 3600, 3, "fan", False, 1),         # 3 ranks
-    (20000, 1920, 4, "fan", False, 1),       # config-4 channel count (25 x 800): two-level with the three-stage level B
+    (20000, 1920, 4, "fan", False, 1),       # config-4 channel count: two-level 25 x 800, shared-memory level B
     (10000, 9600, 2, "fan", True, 3),        # three sub-slabs of 1600 samples per rank (the overlapped schedule's slicing)
     (20000, 3840, 4, "fan", False, 2),       # config-4 channel count, two sub-slabs
 ])
