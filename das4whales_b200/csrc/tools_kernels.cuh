@@ -113,24 +113,31 @@ __host__ __device__ inline double fan_row_blur(const FanParams& p, const double*
     return j1 < j2 ? -v : v;
 }
 
+__host__ __device__ inline double row_blur(const FanParams& p, const double* cw, int i, int j) { return fan_row_blur(p, cw, i, j); }
+
+// The tile and tap bodies below serve every mask whose rows are index intervals before the blur: P supplies nx, ns, r, the
+// weights w / cw and row_blur(p, cw, i, j), the exact axis-1 blur of row i (FanParams here, DesignParams further down).
 // shared copies of the weights, zero-padded to wz[fan_steps(r)], and of cw[2r + 2]
-__host__ __device__ inline void body_fan_weights(const FanParams& p, double* wz, double* cw, int tid, int nthr) {
+template <class P>
+__host__ __device__ inline void body_fan_weights(const P& p, double* wz, double* cw, int tid, int nthr) {
     const int S = fan_steps(p.r);
     for (int s = tid; s < S; s += nthr) wz[s] = s <= 2 * p.r ? p.w[s] : 0.0;
     for (int m = tid; m < 2 * p.r + 2; m += nthr) cw[m] = p.cw[m];
 }
 // CTA (i0, j0): the shared tile H[tr][c] = axis-1 blur at row reflect(i0 - r + tr), column j0 + c
-__host__ __device__ inline void body_fan_fill_tile(const FanParams& p, int i0, int j0, const double* cw, double* H, int tid, int nthr) {
+template <class P>
+__host__ __device__ inline void body_fan_fill_tile(const P& p, int i0, int j0, const double* cw, double* H, int tid, int nthr) {
     const int rows = fan_tile_rows(p.r);
     for (int idx = tid; idx < rows * kFanTJ; idx += nthr) {
         const int tr = idx / kFanTJ, c = idx % kFanTJ, j = j0 + c;
-        H[idx] = j < p.ns ? fan_row_blur(p, cw, reflect_index((long long)i0 - p.r + tr, p.nx), j) : 0.0;
+        H[idx] = j < p.ns ? row_blur(p, cw, reflect_index((long long)i0 - p.r + tr, p.nx), j) : 0.0;
     }
 }
 
 // thread (g, lane): acc[u] = sum_{t = 0..2r} w[t] H[g U + u + t][lane], the axis-0 blur at row i0 + g U + u.  Each tile value
 // is read once and feeds U accumulators; the U weights in flight sit in a register ring (static indices after unrolling).
-__host__ __device__ inline void body_fan_taps(const FanParams& p, const double* wz, const double* H, int g, int lane, double* acc) {
+template <class P>
+__host__ __device__ inline void body_fan_taps(const P& p, const double* wz, const double* H, int g, int lane, double* acc) {
     double wr[kFanU];
 #pragma unroll
     for (int u = 0; u < kFanU; ++u) { acc[u] = 0.0; wr[u] = 0.0; }
@@ -158,6 +165,133 @@ __host__ __device__ inline double fan_unkey(unsigned long long k) {
     double x;
     memcpy(&x, &b, 8);
     return x;
+}
+
+// ---- the hybrid, hybrid_gs and hybrid_ninf_gs masks of dsp.py:174-305, :457-579, :582-702 ---------------------------------
+// Shifted layout: f_j = (j - ns/2) fval, k_i = (i - nx/2) kval as numpy.fft.fftfreq forms them.  col_lo / col_hi are the
+// reference's np.argmax column range (the loop over [col_lo, col_hi) does not run when col_hi <= col_lo).
+//
+// hybrid: elementwise, A[i, j] = H_j c(i, j) inside [col_lo, col_hi) and H_j outside, then A[i, j] + A[i, ns-1-j] (fliplr).
+// hybrid_gs: before the sigma = 20 blur, row i of M + fliplr(M) is 1 on S_i and on its mirror, S_i = {H_j = 1} ∩ ({j in
+// [col_lo, col_hi) : -kp_j < k_i < kp_j} ∪ {j outside [col_lo, col_hi)}), kp_j = f_j / cp_min.  kp_j does not decrease with j
+// (cp_min > 0), so both comparisons first fail and then hold: S_i is the H band cut to [0, col_lo) ∪ [s_i, ns).
+// hybrid_ninf_gs: the blur commutes with fliplr and flipud (a symmetric kernel, 'reflect' mode), so blur(M) + its fliplr, then
+// + its flipud, is the blur of the sum of rows i and nx-1-i of M and their mirrors.  Inside [col_lo, col_hi) M is 1 where
+// k_i > -(f_j / cp_min), a suffix, and k_i < -(f_j / cp_max), a prefix: S_i = H ∩ ([0, col_lo) ∪ [s_i, e_i) ∪ [col_hi, ns)).
+// Each row is a short list of index intervals (overlaps count twice, as the sums do), blurred along axis 1 by interval_blur
+// and along axis 0 by the fan's tile and taps.
+constexpr int kDesignHybrid = 0, kDesignHybridGs = 1, kDesignHybridNinfGs = 2;
+constexpr double kDesignSigma = 20.0;              // ndimage.gaussian_filter(M, 20), dsp.py:540 and :659
+constexpr int kDesignMaxIv = 12;                   // 3 pieces x fliplr x flipud
+constexpr int kDesignStride = 1 + 2 * kDesignMaxIv;  // per row: count, then [a, b) pairs
+
+struct DesignParams {
+    int kind, nx, ns, r;
+    double kval, fval, cs_min, cp_min, cp_max;
+    int col_lo, col_hi, h_lo, h_hi;     // [h_lo, h_hi): where H_j = 1 (gs kinds)
+    const double* H;                    // [ns] (hybrid)
+    const double* w;                    // [2r + 1]
+    const double* cw;                   // [2r + 2]
+    int* iv;                            // [nx][kDesignStride]
+};
+
+// workspace: w[2r + 1], cw[2r + 2], H[ns], then the row intervals
+__host__ __device__ inline size_t design_ws_bytes(int nx, int ns, int r) {
+    return sizeof(double) * ((size_t)(4 * r + 3) + (size_t)ns) + sizeof(int) * (size_t)kDesignStride * (size_t)nx;
+}
+
+// [h_lo, h_hi) = the columns where a gs mask's H is 1; false unless H is 1 on that one band and 0 elsewhere
+__host__ __device__ inline bool design_h_band(const double* H, int ns, int* h_lo, int* h_hi) {
+    int j = 0;
+    while (j < ns && H[j] == 0.0) ++j;
+    *h_lo = j;
+    while (j < ns && H[j] == 1.0) ++j;
+    *h_hi = j;
+    while (j < ns && H[j] == 0.0) ++j;
+    return j == ns;
+}
+
+// the reference's column factor of the hybrid mask (dsp.py:246-262): the -sin ramp, then the sin ramp (both only when
+// ks != kp), then the passband's 1
+__host__ __device__ inline double hybrid_col(double k, double f, double cs_min, double cp_min) {
+    const double ks = f / cs_min, kp = f / cp_min;
+    double c = 0.0;
+    if (ks != kp) {
+        if (k >= -ks && k <= -kp) c = -sin(0.5 * M_PI * (k + ks) / (kp - ks));
+        if (-k >= -ks && -k <= -kp) c = sin(0.5 * M_PI * (k - ks) / (kp - ks));
+    }
+    if (k < kp && k > -kp) c = 1.0;
+    return c;
+}
+
+__host__ __device__ inline double hybrid_half(const DesignParams& p, double k, int j) {
+    const double v = p.H[j];
+    return j >= p.col_lo && j < p.col_hi ? v * hybrid_col(k, (double)(j - p.ns / 2) * p.fval, p.cs_min, p.cp_min) : v;
+}
+
+__host__ __device__ inline double body_hybrid(const DesignParams& p, int i, int j) {
+    const double k = (double)(i - p.nx / 2) * p.kval;
+    return hybrid_half(p, k, j) + hybrid_half(p, k, p.ns - 1 - j);
+}
+
+// which = 0: -kp < k < kp (hybrid_gs); 1: k > -(f / cp_min); 2: not k < -(f / cp_max).  Each first fails, then holds, as j grows.
+__host__ __device__ inline bool design_pred(int which, double k, double f, double cp_min, double cp_max) {
+    if (which == 0) {
+        const double kp = f / cp_min;
+        return k < kp && k > -kp;
+    }
+    if (which == 1) return k > -(f / cp_min);
+    return !(k < -(f / cp_max));
+}
+
+// first j in [lo, hi) where design_pred holds (hi when it never does), by bisection on the reference's comparisons
+__host__ __device__ inline int design_first(int which, int lo, int hi, int ns, double fval, double k, double cp_min, double cp_max) {
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (design_pred(which, k, (double)(mid - ns / 2) * fval, cp_min, cp_max)) hi = mid; else lo = mid + 1;
+    }
+    return lo;
+}
+
+// append [a, b) ∩ H and its fliplr mirror to a row's list
+__host__ __device__ inline void design_push(const DesignParams& p, int* row, int a, int b) {
+    a = a > p.h_lo ? a : p.h_lo;
+    b = b < p.h_hi ? b : p.h_hi;
+    if (a >= b) return;
+    const int n = row[0];
+    row[1 + 2 * n] = a; row[2 + 2 * n] = b;
+    row[3 + 2 * n] = p.ns - b; row[4 + 2 * n] = p.ns - a;
+    row[0] = n + 2;
+}
+
+// S_m (row m of M before the blur) and its mirror, appended to row
+__host__ __device__ inline void design_row_set(const DesignParams& p, int m, int* row) {
+    const double k = (double)(m - p.nx / 2) * p.kval;
+    const int lo = p.col_lo, hi = p.col_hi > lo ? p.col_hi : lo;
+    design_push(p, row, 0, lo);
+    if (p.kind == kDesignHybridGs) {
+        design_push(p, row, design_first(0, lo, hi, p.ns, p.fval, k, p.cp_min, p.cp_max), p.ns);
+    } else {
+        design_push(p, row, design_first(1, lo, hi, p.ns, p.fval, k, p.cp_min, p.cp_max),
+                    design_first(2, lo, hi, p.ns, p.fval, k, p.cp_min, p.cp_max));
+        design_push(p, row, hi, p.ns);
+    }
+}
+
+// row i's interval list: S_i for hybrid_gs; S_i and S_{nx-1-i} for hybrid_ninf_gs (the flipud partner; itself at an odd nx's
+// centre row, which the sum counts twice)
+__host__ __device__ inline void body_design_row(const DesignParams& p, int i) {
+    int* row = p.iv + (size_t)i * kDesignStride;
+    row[0] = 0;
+    design_row_set(p, i, row);
+    if (p.kind == kDesignHybridNinfGs) design_row_set(p, p.nx - 1 - i, row);
+}
+
+__host__ __device__ inline double row_blur(const DesignParams& p, const double* cw, int i, int j) {
+    const int* row = p.iv + (size_t)i * kDesignStride;
+    double v = 0.0;
+    for (int q = 0; q < row[0]; ++q) v += interval_blur(cw, p.r, p.ns, row[1 + 2 * q], row[2 + 2 * q], j);
+    return v;
 }
 
 // ---- per-row moments over time chunks, and the linear detrend --------------------------------------------------------------

@@ -355,6 +355,20 @@ int d4w_fan_blur(float* dev_out, int nx, int ns, double kval, double fval, doubl
                  void* dev_workspace, void* stream);
 int d4w_row_moments(const float* dev_x, size_t ld, int nrows, int n, int chunk, double* dev_out, void* stream);
 int d4w_detrend_linear(const float* dev_x, size_t ld, int nrows, int n, const double* dev_moments, float* dev_y, void* stream);
+
+/* ---- the hybrid masks of dsp.py designed on the device, as float32 [nx][ns] in the reference's shifted layout, to hand to
+ * d4w_fk_mask_create_dense.  kind 0: hybrid_filter_design (dsp.py:174-305), elementwise in float64; kind 1:
+ * hybrid_gs_filter_design (:457-579); kind 2: hybrid_ninf_gs_filter_design (:582-702).  Kinds 1 and 2 are blurred as
+ * scipy.ndimage.gaussian_filter(M, 20) (truncate 4, mode 'reflect') in float64, with no normalisation.  f_j = (j - ns/2) fval,
+ * k_i = (i - nx/2) kval (numpy.fft.fftfreq's products); host_H = the design function's ns-long H (host pointer, read
+ * before the call returns; for kinds 1 and 2 it must be 1 on one band of columns and 0 elsewhere); col_lo / col_hi = its
+ * np.argmax column range (col_hi < col_lo: the reference's loop does not run; kind 0 needs col_lo <= col_hi).  D4W_ERR_ARG
+ * unless the speeds are finite and > 0, fval finite and > 0, kval finite and fmin < fmax finite; nx <= 65 535.
+ * cp_max is read by kind 2 only, cs_min by kind 0 only.  dev_workspace: d4w_mask_design_workspace_bytes(nx, ns). */
+size_t d4w_mask_design_workspace_bytes(int nx, int ns);
+int d4w_mask_design(int kind, float* dev_out, int nx, int ns, double kval, double fval, double cs_min, double cp_min,
+                    double cp_max, double fmin, double fmax, int col_lo, int col_hi, const double* host_H,
+                    void* dev_workspace, void* stream);
 /* D4W_CDEF_END */
 
 #ifdef __cplusplus

@@ -103,11 +103,36 @@ def _shifted_axes(trace_shape, selected_channels, dx, fs):
     return freq, knum
 
 
-def hybrid_filter_design(trace_shape, selected_channels, dx, fs, cs_min=1400., cp_min=1450., fmin=15., fmax=25.,
-                         display_filter=False):
-    """Infinite-speed hybrid mask, sine tapers in f and k (reference: dsp.py:174-305).  Built on the
-    host at design time (vectorised) and applied through the dense-mask GPU path."""
-    freq, knum = _shifted_axes(trace_shape, selected_channels, dx, fs)
+def _design_steps(trace_shape, selected_channels, dx, fs, speeds, fmin, fmax):
+    """(kval, fval) when the device design covers the arguments, else None: positive finite speeds, finite fmin < fmax,
+    numpy's fftfreq steps finite with fval > 0 (the shifted frequency axis then increases, which the interval argument of
+    csrc/tools_kernels.cuh needs) and at most 65 535 channels."""
+    try:
+        kval, fval = _fftfreq_steps(trace_shape, selected_channels, dx, fs)
+        vals = np.array([float(v) for v in speeds] + [float(fmin), float(fmax), kval, fval])
+        nx, ns = (int(n) for n in trace_shape)
+    except (ZeroDivisionError, TypeError, ValueError, OverflowError):
+        return None
+    if not (np.isfinite(vals).all() and (vals[:len(speeds)] > 0).all() and fmin < fmax and fval > 0 and 1 <= nx <= 65535
+            and ns >= 1):
+        return None
+    return kval, fval
+
+
+def _designed_mask(kind, host, trace_shape, selected_channels, dx, fs, speeds, fmin, fmax, H, col_lo, col_hi):
+    """The lazy mask designed on the device (fk.DESIGN_KINDS), or FkMask.from_dense(host()) for arguments outside its domain.
+    speeds = (cs_min, cp_min, cp_max): the ones the design function takes, cp_max = None when it takes none."""
+    steps = _design_steps(trace_shape, selected_channels, dx, fs, [c for c in speeds if c is not None], fmin, fmax)
+    if steps is None or (kind == "hybrid" and col_hi < col_lo):
+        return _fk.FkMask.from_dense(host())
+    cs_min, cp_min, cp_max = speeds
+    return _fk.FkMask(kind, trace_shape, dict(kval=steps[0], fval=steps[1], cs_min=float(cs_min), cp_min=float(cp_min),
+                                              cp_max=float(cp_min if cp_max is None else cp_max), fmin=float(fmin),
+                                              fmax=float(fmax), H=H, col_lo=int(col_lo), col_hi=int(col_hi)),
+                      order="C", host=host)
+
+
+def _hybrid_H(freq, fmin, fmax):
     fpmin, fpmax = fmin - 4, fmax + 4                          # df_taper = 4 Hz (dsp.py:216)
     H = np.zeros_like(freq)
     up = (freq >= fpmin) & (freq <= fmin)
@@ -115,7 +140,12 @@ def hybrid_filter_design(trace_shape, selected_channels, dx, fs, cs_min=1400., c
     H[(freq >= fmin) & (freq <= fmax)] = 1
     dn = (freq >= fmax) & (freq <= fpmax)
     H[dn] = np.cos(0.5 * np.pi * (freq[dn] - fmax) / (fmax - fpmax))
-    lo, hi = int(np.argmax(freq >= fpmin)), int(np.argmax(freq >= fpmax))
+    return H, int(np.argmax(freq >= fpmin)), int(np.argmax(freq >= fpmax))
+
+
+def _hybrid_host(trace_shape, selected_channels, dx, fs, cs_min, cp_min, fmin, fmax):
+    freq, knum = _shifted_axes(trace_shape, selected_channels, dx, fs)
+    H, lo, hi = _hybrid_H(freq, fmin, fmax)
     f = freq[lo:hi][None, :]
     k = knum[:, None]
     ks, kp = f / cs_min, f / cp_min
@@ -128,46 +158,74 @@ def hybrid_filter_design(trace_shape, selected_channels, dx, fs, cs_min=1400., c
     col = np.where((k < kp) & (k > -kp), 1.0, col)
     M = np.tile(H, (len(knum), 1))
     M[:, lo:hi] *= col
-    M = M + M[:, ::-1]                                         # np.fliplr symmetrisation (dsp.py:264)
-    mask = _fk.FkMask.from_dense(M)
+    return M + M[:, ::-1]                                      # np.fliplr symmetrisation (dsp.py:264)
+
+
+def hybrid_filter_design(trace_shape, selected_channels, dx, fs, cs_min=1400., cp_min=1450., fmin=15., fmax=25.,
+                         display_filter=False):
+    """Infinite-speed hybrid mask, sine tapers in f and k (reference: dsp.py:174-305).  Returns a lazy `FkMask` at once:
+    the filter designs it on the device (d4w_mask_design), `np.asarray` / `todense()` build the float64 matrix on the host."""
+    freq, knum = _shifted_axes(trace_shape, selected_channels, dx, fs)
+    H, lo, hi = _hybrid_H(freq, fmin, fmax)
+    mask = _designed_mask("hybrid", lambda: _hybrid_host(trace_shape, selected_channels, dx, fs, cs_min, cp_min, fmin, fmax),
+                          trace_shape, selected_channels, dx, fs, (cs_min, cp_min, None), fmin, fmax, H, lo, hi)
     if display_filter:
         _display_mask(mask, freq, knum)
     return mask
+
+
+def _gs_H(freq, fmin, fmax):
+    H = np.zeros_like(freq)
+    H[(freq >= fmin) & (freq <= fmax)] = 1
+    return H, int(np.argmax(freq >= fmin - 4)), int(np.argmax(freq >= fmax + 4))
 
 
 def _gs_start(trace_shape, selected_channels, dx, fs, fmin, fmax):
     freq, knum = _shifted_axes(trace_shape, selected_channels, dx, fs)
-    H = np.zeros_like(freq)
-    H[(freq >= fmin) & (freq <= fmax)] = 1
-    lo, hi = int(np.argmax(freq >= fmin - 4)), int(np.argmax(freq >= fmax + 4))
+    H, lo, hi = _gs_H(freq, fmin, fmax)
     return freq, knum, np.tile(H, (len(knum), 1)), lo, hi
 
 
-def hybrid_gs_filter_design(trace_shape, selected_channels, dx, fs, cs_min=1400., cp_min=1450., fmin=15., fmax=25.,
-                            display_filter=False):
-    """Infinite-speed hybrid mask with Gaussian (sigma = 20 bins) tapers (reference: dsp.py:457-579)."""
+def _hybrid_gs_host(trace_shape, selected_channels, dx, fs, fmin, fmax, cp_min):
     from scipy import ndimage
     freq, knum, M, lo, hi = _gs_start(trace_shape, selected_channels, dx, fs, fmin, fmax)
     kp = freq[lo:hi][None, :] / cp_min
     M[:, lo:hi] *= ((knum[:, None] < kp) & (knum[:, None] > -kp))
-    M = ndimage.gaussian_filter(M + M[:, ::-1], 20)            # dsp.py:539-540
-    mask = _fk.FkMask.from_dense(M)
+    return ndimage.gaussian_filter(M + M[:, ::-1], 20)         # dsp.py:539-540
+
+
+def hybrid_gs_filter_design(trace_shape, selected_channels, dx, fs, cs_min=1400., cp_min=1450., fmin=15., fmax=25.,
+                            display_filter=False):
+    """Infinite-speed hybrid mask with Gaussian (sigma = 20 bins) tapers (reference: dsp.py:457-579).  Returns a lazy
+    `FkMask` at once: designed on the device for the filter, on the host (scipy.ndimage) for `np.asarray` / `todense()`."""
+    freq, knum = _shifted_axes(trace_shape, selected_channels, dx, fs)
+    H, lo, hi = _gs_H(freq, fmin, fmax)
+    mask = _designed_mask("hybrid_gs", lambda: _hybrid_gs_host(trace_shape, selected_channels, dx, fs, fmin, fmax, cp_min),
+                          trace_shape, selected_channels, dx, fs, (cs_min, cp_min, None), fmin, fmax, H, lo, hi)
     if display_filter:
         _display_mask(mask, freq, knum)
     return mask
 
 
-def hybrid_ninf_gs_filter_design(trace_shape, selected_channels, dx, fs, cs_min=1400., cp_min=1450., cp_max=3400,
-                                 cs_max=3500, fmin=15., fmax=25., display_filter=False):
-    """Finite-speed hybrid mask with Gaussian tapers (reference: dsp.py:582-702)."""
+def _hybrid_ninf_gs_host(trace_shape, selected_channels, dx, fs, fmin, fmax, cp_min, cp_max):
     from scipy import ndimage
     freq, knum, M, lo, hi = _gs_start(trace_shape, selected_channels, dx, fs, fmin, fmax)
     f = freq[lo:hi][None, :]
     M[:, lo:hi] *= ((knum[:, None] > -f / cp_min) & (knum[:, None] < -f / cp_max))
     M = ndimage.gaussian_filter(M, 20)                         # dsp.py:659
     M = M + M[:, ::-1]
-    M = M + M[::-1, :]
-    mask = _fk.FkMask.from_dense(M)
+    return M + M[::-1, :]
+
+
+def hybrid_ninf_gs_filter_design(trace_shape, selected_channels, dx, fs, cs_min=1400., cp_min=1450., cp_max=3400,
+                                 cs_max=3500, fmin=15., fmax=25., display_filter=False):
+    """Finite-speed hybrid mask with Gaussian tapers (reference: dsp.py:582-702).  Returns a lazy `FkMask` at once:
+    designed on the device for the filter, on the host (scipy.ndimage) for `np.asarray` / `todense()`."""
+    freq, knum = _shifted_axes(trace_shape, selected_channels, dx, fs)
+    H, lo, hi = _gs_H(freq, fmin, fmax)
+    mask = _designed_mask("hybrid_ninf_gs",
+                          lambda: _hybrid_ninf_gs_host(trace_shape, selected_channels, dx, fs, fmin, fmax, cp_min, cp_max),
+                          trace_shape, selected_channels, dx, fs, (cs_min, cp_min, cp_max), fmin, fmax, H, lo, hi)
     if display_filter:
         _display_mask(mask, freq, knum)
     return mask

@@ -97,14 +97,20 @@ class _DeviceMask:
         weakref.finalize(self, L.d4w_fk_mask_destroy, self.ptr)
 
 
+# the masks designed on the device as a float32 plane (d4w_mask_design's kind codes); the filter takes them through the dense
+# route, and todense() runs the host restatement the design function passed in
+DESIGN_KINDS = {"hybrid": 0, "hybrid_gs": 1, "hybrid_ninf_gs": 2}
+
+
 class FkMask:
     """Lazy f-k mask: the closed-form description of what the reference's design function
     returns.  `np.asarray(mask)` / `mask.todense()` materialise exactly the reference's
     [channel x time] float64 array (shifted layout) on demand; `fk_filter_filt` uses the
-    description directly and never builds the dense matrix.
+    description directly and never builds the dense matrix.  For the DESIGN_KINDS the filter's
+    table comes from a plane designed on the device, and todense() runs the host design (`host`).
     """
 
-    def __init__(self, kind, shape, params, order="C"):
+    def __init__(self, kind, shape, params, order="C", host=None):
         self.kind = kind
         self.shape = (int(shape[0]), int(shape[1]))
         self.params = params
@@ -114,6 +120,7 @@ class FkMask:
         self.dtype = np.dtype(np.float64)
         self._dev = {}
         self._dense = None
+        self._host = host              # designed kinds: the host restatement todense() runs (and caches) on demand
 
     # ---- device side -------------------------------------------------------------------
     def _create(self, L, out, plan):
@@ -130,16 +137,38 @@ class FkMask:
         else:
             raise ValueError(f"unknown analytic mask kind {self.kind}")
 
+    def _design_plane(self, plan):
+        """float32 [nx, ns] device plane of a designed kind (d4w_mask_design), for the dense support scan and table."""
+        if (plan.nx, plan.ns) != self.shape:
+            raise ValueError(f"operands could not be broadcast together with shapes ({plan.nx},{plan.ns}) {self.shape}")
+        torch = _torch()
+        L = _lib.lib()
+        p = self.params
+        nx, ns = self.shape
+        h = np.ascontiguousarray(p["H"], dtype=np.float64)
+        with torch.cuda.device(plan.device):
+            out = torch.empty((nx, ns), dtype=torch.float32, device=f"cuda:{plan.device}")
+            ws = torch.empty(int(L.d4w_mask_design_workspace_bytes(nx, ns)), dtype=torch.uint8, device=f"cuda:{plan.device}")
+            _lib.check(L.d4w_mask_design(DESIGN_KINDS[self.kind], _lib.ptr(out, "float*"), nx, ns, p["kval"], p["fval"],
+                                         p["cs_min"], p["cp_min"], p["cp_max"], p["fmin"], p["fmax"], p["col_lo"], p["col_hi"],
+                                         _lib.ffi.cast("double*", h.ctypes.data), _lib.ptr(ws), _lib.stream_ptr()),
+                       f"{self.kind} mask design")
+        return out
+
+    def _new_device_mask(self, plan, eps=0.0):
+        if self.kind == "dense":      # caller-supplied planes, and designs outside the device route's domain
+            return _DenseMaskHolder(plan, _dense_to_device(self._dense, plan.device), eps).dm
+        if self.kind in DESIGN_KINDS:  # designed into a transient plane on the device, then scanned like a dense mask
+            return _DenseMaskHolder(plan, self._design_plane(plan), eps).dm
+        return _DeviceMask(plan, self._create, eps)
+
     def on_device(self, plan, eps=0.0):
         eps = float(eps or 0.0)
         if eps:
             key = (plan.serial, eps)
             dm = self._dev.get(key)
             if dm is None:
-                if self.kind == "dense":
-                    dm = _DenseMaskHolder(plan, _dense_to_device(self._dense, plan.device), eps).dm
-                else:
-                    dm = _DeviceMask(plan, self._create, eps)
+                dm = self._new_device_mask(plan, eps)
                 self._dev[key] = dm
             return dm
         dm = self._dev.get(plan.serial)
@@ -148,10 +177,7 @@ class FkMask:
                 del self._dev[k]                      # tables of plans that were dropped by free_plans()
             if (plan.nx, plan.ns) != self.shape:
                 raise ValueError(f"operands could not be broadcast together with shapes ({plan.nx},{plan.ns}) {self.shape}")
-            if self.kind == "dense":      # design functions without a closed form on the device
-                dm = _DenseMaskHolder(plan, _dense_to_device(self._dense, plan.device)).dm
-            else:
-                dm = _DeviceMask(plan, self._create)
+            dm = self._new_device_mask(plan)
             self._dev[plan.serial] = dm
         return dm
 
@@ -165,6 +191,8 @@ class FkMask:
 
     # ---- host side (what plots / prints see) -------------------------------------------
     def todense(self):
+        if self._dense is None and self._host is not None:
+            self._dense = self._host()
         if self._dense is None:
             torch = _torch()
             L = _lib.lib()

@@ -298,7 +298,8 @@ class FkCompPipeline(_FilePipeline):
         inf_gs   dsp.hybrid_gs_filter_design        (:92-95, cs_min and cp_min only)
 
     then the argmax of inf_cos, its cross-section at that time (:104-106) and snr_tr_array(env=True) of each output
-    (:113-122).  The masks are designed once, here."""
+    (:113-122).  The masks are designed once, here, on the device (d4w_mask_design for the hybrid, hybrid_gs and
+    hybrid_ninf_gs masks): construction takes milliseconds, and no float64 mask plane is built on the host."""
 
     _hybrid_ninf_front_end = False
 
