@@ -11,6 +11,7 @@
 #include "d4w_common.hpp"
 #include "fk_hostplan.hpp"
 #include "fk_kernels.cuh"
+#include "fk_spectrum.cuh"
 
 using namespace d4w;
 
@@ -21,6 +22,9 @@ std::atomic<long long>& launch_counter() { static std::atomic<long long> c{0}; r
 int launch_row_mid_oop(bool dual, bool fused, dim3 grid, int threads, size_t smem, const RowParams& rp, float2* w, size_t ldw,
                        const float* tab, size_t tab_slot_stride, int nslots, float2* dst, int device, cudaStream_t stream);
 int launch_bank_gather(const float* src, float* dst, const int* src_row, int ns, size_t total, cudaStream_t stream);
+// f-k spectrum power pass (d4w_fk_spectrum.cu)
+int launch_fk_power(dim3 grid, int threads, size_t smem, const RowParams& rp, const SpecParams& sp, const float2* w, size_t ldw,
+                    float* out, int device, cudaStream_t stream);
 }  // namespace d4w
 
 extern "C" const char* d4w_last_error(void) { return last_error_ref().c_str(); }
@@ -894,4 +898,89 @@ extern "C" int d4w_fk_bank_apply(d4w_fk_plan* pl, d4w_fk_bank* b, const float* x
     for (int i = 0; rc == D4W_OK && b && i < (int)b->masks.size(); ++i)
         for (int pass = 3; rc == D4W_OK && pass <= 5; ++pass) rc = d4w_fk_bank_apply_pass(pl, b, x, ys, ws, taper, pass, i, stream);
     return rc;
+}
+
+// ------------------------------------------------------------------------------- f-k power spectrum
+// |fftshift(fft2(x))|^2 over a band of the shifted plane: P1 and P2 of the filter on the band's half-plane rows, then the
+// forward-only power pass (fk_spectrum.cuh) in place of P3's mask multiply and inverse; no P4 or P5.  The rows are the
+// k' in [0, nx/2] with +k' or -k' inside the band, kept in a support object (slot and column tables, no mask table) as
+// a mask bank keeps its union support.
+struct d4w_fk_spectrum {
+    d4w_fk_plan* plan = nullptr;
+    d4w_fk_mask* sup = nullptr;
+    int k_lo = 0, k_hi = 0, f_lo = 0, f_hi = 0;
+    int* d_k2pos_row = nullptr;               // natural T2-point frequency -> position after the forward stages
+};
+
+extern "C" int d4w_fk_spectrum_destroy(d4w_fk_spectrum* s) {
+    if (!s) return D4W_OK;
+    DeviceGuard guard(s->plan->device);
+    d4w_fk_mask_destroy(s->sup);
+    cudaFree(s->d_k2pos_row);
+    delete s;
+    return D4W_OK;
+}
+
+extern "C" int d4w_fk_spectrum_create(d4w_fk_spectrum** out, d4w_fk_plan* plan, int k_lo, int k_hi, int f_lo, int f_hi) {
+    if (!out) return fail(D4W_ERR_ARG, "d4w_fk_spectrum_create: null output pointer");
+    *out = nullptr;
+    if (!plan) return fail(D4W_ERR_ARG, "d4w_fk_spectrum_create: null plan");
+    const int nx = plan->nx, ns = plan->ns;
+    if (k_lo < 0 || k_hi > nx || k_lo >= k_hi)
+        return fail(D4W_ERR_ARG, "d4w_fk_spectrum_create: wavenumber rows [" + std::to_string(k_lo) + ", " + std::to_string(k_hi) +
+                                     ") empty or outside [0, " + std::to_string(nx) + ")");
+    if (f_lo < 0 || f_hi > ns || f_lo >= f_hi)
+        return fail(D4W_ERR_ARG, "d4w_fk_spectrum_create: frequency columns [" + std::to_string(f_lo) + ", " + std::to_string(f_hi) +
+                                     ") empty or outside [0, " + std::to_string(ns) + ")");
+    DeviceGuard guard(plan->device);
+    std::vector<int> rows;
+    for (int k = 0; k <= nx / 2; ++k) {
+        const int rp = (k + nx / 2) % nx, rn = (nx - k + nx / 2) % nx;
+        if ((rp >= k_lo && rp < k_hi) || (rn >= k_lo && rn < k_hi)) rows.push_back(k);
+    }
+    const std::vector<int>& p2k = plan->hostplan.pos2k_row;
+    std::vector<int> k2p(p2k.size());
+    for (size_t p = 0; p < p2k.size(); ++p) k2p[p2k[p]] = (int)p;
+    auto s = new d4w_fk_spectrum();
+    s->plan = plan; s->k_lo = k_lo; s->k_hi = k_hi; s->f_lo = f_lo; s->f_hi = f_hi;
+    s->sup = new d4w_fk_mask();
+    s->sup->plan = plan; s->sup->device = plan->device;
+    int rc = build_support_tables(s->sup, rows);
+    if (rc == D4W_OK) {
+        cudaError_t e = upload(&s->d_k2pos_row, k2p);
+        if (e != cudaSuccess) rc = fail(D4W_ERR_CUDA, std::string("spectrum frequency map: ") + cudaGetErrorString(e));
+    }
+    if (rc != D4W_OK) { d4w_fk_spectrum_destroy(s); return rc; }
+    *out = s;
+    return D4W_OK;
+}
+
+extern "C" int d4w_fk_spectrum_rows(const d4w_fk_spectrum* s) { return s ? s->sup->nact : 0; }
+
+extern "C" size_t d4w_fk_spectrum_workspace_bytes(const d4w_fk_plan* pl, const d4w_fk_spectrum* s) {
+    if (!pl || !s) return 0;
+    return kept_rows_bytes(pl, s->sup->nact) + col2_ring_bytes(pl);
+}
+
+extern "C" int d4w_fk_spectrum_apply(d4w_fk_plan* pl, d4w_fk_spectrum* s, const float* x, float* out, void* ws, int taper,
+                                     float scale, int accumulate, void* stream_v) {
+    if (!pl || !s || !x || !out || !ws) return fail(D4W_ERR_ARG, "d4w_fk_spectrum_apply: null argument");
+    if (s->plan->device != pl->device) return fail(D4W_ERR_ARG, "d4w_fk_spectrum_apply: plan and spectrum live on different devices");
+    if (s->plan != pl) return fail(D4W_ERR_ARG, "d4w_fk_spectrum_apply: spectrum was made for a different plan");
+    if (accumulate != 0 && accumulate != 1) return fail(D4W_ERR_ARG, "d4w_fk_spectrum_apply: accumulate must be 0 or 1");
+    if (check_matrix_alignment(x, pl->ns, "d4w_fk_spectrum_apply: input") != D4W_OK) return D4W_ERR_ARG;
+    DeviceGuard guard(pl->device);
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    const d4w_fk_mask* sup = s->sup;
+    const int nact = sup->nact;
+    float2* w = (float2*)ws;
+    cpd* v2 = use_two_level(pl, sup, ws) ? reinterpret_cast<cpd*>((char*)ws + kept_rows_bytes(pl, nact)) : nullptr;
+    int rc = fk_run_pass(pl, sup, x, nullptr, w, v2, nullptr, nullptr, taper ? pl->d_taper : nullptr, 1, nact, stream);
+    if (rc == D4W_OK) rc = fk_run_pass(pl, sup, nullptr, nullptr, w, v2, nullptr, nullptr, nullptr, 2, nact, stream);
+    if (rc != D4W_OK) return rc;
+    SpecParams sp{};
+    sp.act_k = sup->d_act_k; sp.k2pos_row = s->d_k2pos_row; sp.nx = pl->nx; sp.ns = pl->ns;
+    sp.k_lo = s->k_lo; sp.k_hi = s->k_hi; sp.f_lo = s->f_lo; sp.f_hi = s->f_hi; sp.scale = scale; sp.accumulate = accumulate;
+    return launch_fk_power(dim3(pl->t1, nact), pl->row_threads, pl->row_smem, pl->row, sp, w, (size_t)pl->ns, out, pl->device,
+                           stream);
 }

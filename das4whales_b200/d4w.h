@@ -140,6 +140,26 @@ int d4w_fk_bank_apply(d4w_fk_plan* plan, d4w_fk_bank* bank, const float* dev_x, 
 int d4w_fk_bank_apply_pass(d4w_fk_plan* plan, d4w_fk_bank* bank, const float* dev_x, float* const* dev_ys,
                            void* dev_workspace, int taper, int pass, int mask, void* stream);
 
+/* ---- f-k power spectrum: P = |fftshift(fft2(x))|^2 over a band of the shifted plane, the filter's forward
+ *      transform (P1, P2) followed by a forward-only power pass; no mask, no inverse ----------------------------- */
+typedef struct d4w_fk_spectrum d4w_fk_spectrum;
+/* The band is rows [k_lo, k_hi) x columns [f_lo, f_hi) of the shifted [nx x ns] plane (half-open).  Only the
+ * half-plane rows k' in [0, nx/2] with +k' or -k' inside the band are transformed.  D4W_ERR_ARG: an empty band or one
+ * outside the plane, a null argument.  The spectrum keeps a reference to `plan`, which must outlive it. */
+int    d4w_fk_spectrum_create(d4w_fk_spectrum** out, d4w_fk_plan* plan, int k_lo, int k_hi, int f_lo, int f_hi);
+int    d4w_fk_spectrum_destroy(d4w_fk_spectrum* s);
+/* half-plane rows transformed */
+int    d4w_fk_spectrum_rows(const d4w_fk_spectrum* s);
+/* bytes of workspace for d4w_fk_spectrum_apply: the transformed rows, plus the level-A/B intermediate of a
+ * two-level plan */
+size_t d4w_fk_spectrum_workspace_bytes(const d4w_fk_plan* plan, const d4w_fk_spectrum* s);
+/* dev_out[(k_hi - k_lo) x (f_hi - f_lo)] float32 = scale * P (accumulate = 0) or += scale * P (accumulate = 1), P the
+ * band of |fftshift(fft2(x))|^2, x tapered first by Tukey(alpha=0.03) along time when taper != 0 (x itself is not
+ * modified).  x: float32 [nx x ns], aligned as d4w_fk_apply requires.  D4W_ERR_ARG: a null argument, a misaligned
+ * x, a spectrum made for another plan or device. */
+int    d4w_fk_spectrum_apply(d4w_fk_plan* plan, d4w_fk_spectrum* s, const float* dev_x, float* dev_out,
+                             void* dev_workspace, int taper, float scale, int accumulate, void* stream);
+
 /* ---- generic shared-memory FFT plan (matched-filter blocks, STFT frames) ----------------- */
 typedef struct d4w_fft_plan d4w_fft_plan;
 typedef struct d4w_row_plan d4w_row_plan;

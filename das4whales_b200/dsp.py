@@ -330,6 +330,55 @@ def fk_filter_filts(trace, fk_filter_matrices, tapering=False):
     return [_to_host64(y) for y in ys]
 
 
+def _band(axis, lo, hi, what):
+    """Half-open index range of {i : lo <= axis[i] <= hi} (a contiguous run: the shifted axes are monotonic)."""
+    idx = np.flatnonzero((axis >= lo) & (axis <= hi))
+    if idx.size == 0:
+        raise ValueError(f"fk_spectrum: {what} selects no bin of the axis [{axis[0]}, {axis[-1]}]")
+    return int(idx[0]), int(idx[-1]) + 1
+
+
+def fk_spectrum(trace, selected_channels, dx, fs, f_range=(0., np.inf), k_range=(-np.inf, np.inf), nperseg=None,
+                tapering=False):
+    """f-k power spectrum P = |fftshift(fft2(trace))|^2 over a frequency and wavenumber band, unnormalised, on the
+    axes the mask designs use: knum = fftshift(fftfreq(nx, selected_channels[2] * dx)) and
+    freq = fftshift(fftfreq(n, 1 / fs)), n the record length or `nperseg`.  Returns (P, f, k): P [len(k), len(f)],
+    f = freq[f_range[0] <= freq <= f_range[1]] and k = knum[k_range[0] <= knum <= k_range[1]] (float64 ndarrays).
+
+    The default band is numpy's non-negative frequencies (for even n the Nyquist bin sits at -fs/2 and is left out;
+    a negative f_range[0] takes it) and every wavenumber.  nperseg=L: the mean of the spectra of the ns // L whole
+    blocks trace[:, b*L:(b+1)*L] (a trailing partial block is not used).  tapering=True multiplies each block by
+    Tukey(n, alpha=0.03) along time, as taper_data does, but never modifies the caller's array.  An ndarray gives a
+    float64 P, a CUDA tensor a float32 CUDA tensor.  Shapes ([nx, ns], or [nx, nperseg]) follow the f-k filter's rules
+    (supported_shape); an unsupported one raises ValueError."""
+    if _is_tensor(trace):
+        if trace.dim() != 2 or trace.is_complex():
+            raise ValueError(f"fk_spectrum: expected a real 2-D [channel x time] array, got {tuple(trace.shape)} {trace.dtype}")
+        x = _to_device(trace)
+    else:
+        arr = np.asarray(trace)
+        if arr.ndim != 2 or np.iscomplexobj(arr):
+            raise ValueError(f"fk_spectrum: expected a real 2-D [channel x time] array, got {arr.shape} {arr.dtype}")
+        x = None
+    nx, ns = (int(v) for v in trace.shape)
+    n = ns
+    if nperseg is not None:
+        n = int(nperseg)
+        if n < 1 or n > ns:
+            raise ValueError(f"fk_spectrum: nperseg = {nperseg} must lie in [1, {ns}]")
+    knum = np.fft.fftshift(np.fft.fftfreq(nx, selected_channels[2] * dx))
+    freq = np.fft.fftshift(np.fft.fftfreq(n, 1 / fs))
+    f_idx = _band(freq, f_range[0], f_range[1], f"f_range {tuple(f_range)}")
+    k_idx = _band(knum, k_range[0], k_range[1], f"k_range {tuple(k_range)}")
+    device = x.device.index if x is not None else _fk._torch().cuda.current_device()
+    spec = _fk.FkSpectrum((nx, n), k_idx, f_idx, device=device)
+    if x is None:
+        x = _to_device(arr)
+    p = spec(x, tapering=tapering)
+    f, k = freq[f_idx[0]:f_idx[1]], knum[k_idx[0]:k_idx[1]]
+    return (p if _is_tensor(trace) else _to_host64(p)), f, k
+
+
 # ------------------------------------------------------------------------------ IIR
 def butterworth_filter(filterspec, fs):
     """SOS Butterworth design (reference: dsp.py:789-827) -- design only, host side."""

@@ -1,6 +1,7 @@
 """Host side of the f-k filter: mask descriptors (`FkMask`), per-shape plans and the reusable
 `FkFilter` object that owns the device buffers.  dsp.fk_filter_design / hybrid_*_filter_design
-return `FkMask`; dsp.fk_filter_filt / fk_filter_sparsefilt run an `FkFilter`.
+return `FkMask`; dsp.fk_filter_filt / fk_filter_sparsefilt run an `FkFilter`; dsp.fk_spectrum runs an
+`FkSpectrum` (the same forward transform, ending in |X|^2 over a band).
 
 All arithmetic happens in libd4w.so (hand-written sm_90a CUDA, see csrc/fk_kernels.cuh);
 PyTorch is used for device memory and streams only.
@@ -473,3 +474,72 @@ class FkFilterBank:
     def traffic_bytes(self):
         """HBM bytes each pass must move for the whole bank (passes 3..5 summed over the masks)."""
         return _traffic_bytes(self.plan, self.rows_kept, len(self.dms))
+
+
+def _destroy_spectrum(lib, ptr, plan):
+    """Destroy a d4w_fk_spectrum; `plan` is held until then, since the spectrum points to it."""
+    lib.d4w_fk_spectrum_destroy(ptr)
+
+
+class FkSpectrum:
+    """f-k power spectrum |fftshift(fft2(x))|^2 over one band of one matrix shape (d4w_fk_spectrum): the filter's
+    forward transform on the half-plane wavenumber rows that touch the band, then a forward-only power pass.
+
+    >>> spec = FkSpectrum((nx, ns), (k0, k1), (f0, f1), device=0)   # half-open index ranges on the shifted axes
+    >>> p = spec(x_cuda)             # float32 [k1 - k0, f1 - f0]
+    >>> p = spec(x_long)             # x_long [nx, m >= ns]: mean over the m // ns whole blocks of ns samples
+
+    `rows` is the number of half-plane rows k' in [0, nx/2] transformed (those with +k' or -k' inside the band)."""
+
+    def __init__(self, shape, k_idx, f_idx, device=None):
+        torch = _torch()
+        self.device = torch.cuda.current_device() if device is None else int(device)
+        self.plan = get_plan(int(shape[0]), int(shape[1]), self.device)
+        self.k_idx = (int(k_idx[0]), int(k_idx[1]))
+        self.f_idx = (int(f_idx[0]), int(f_idx[1]))
+        self.shape = (self.k_idx[1] - self.k_idx[0], self.f_idx[1] - self.f_idx[0])
+        L = _lib.lib()
+        out = _lib.ffi.new("d4w_fk_spectrum**")
+        with torch.cuda.device(self.device):
+            _lib.check(L.d4w_fk_spectrum_create(out, self.plan.ptr, *self.k_idx, *self.f_idx), "fk spectrum")
+        self.ptr = out[0]
+        weakref.finalize(self, _destroy_spectrum, L, self.ptr, self.plan)
+        self.rows = int(L.d4w_fk_spectrum_rows(self.ptr))
+        self.workspace_bytes = int(L.d4w_fk_spectrum_workspace_bytes(self.plan.ptr, self.ptr))
+
+    def _ws(self):
+        return self.plan.get_workspace(self.workspace_bytes)
+
+    def __call__(self, x, out=None, tapering=False):
+        """Spectrum of x [nx, ns], or the mean of the spectra of the m // ns whole blocks x[:, b*ns:(b+1)*ns] of
+        x [nx, m] (a trailing partial block is not used).  tapering=True: each block is multiplied by
+        Tukey(ns, alpha=0.03) along time first; x is never modified."""
+        torch = _torch()
+        nx, ns = self.plan.nx, self.plan.ns
+        if x.dtype != torch.float32 or not x.is_cuda or not x.is_contiguous() or x.dim() != 2:
+            raise ValueError("FkSpectrum expects a contiguous 2-D float32 CUDA tensor")
+        if x.shape[0] != nx or x.shape[1] < ns:
+            raise ValueError(f"FkSpectrum built for blocks of {(nx, ns)}, got {tuple(x.shape)}")
+        if out is None:
+            out = torch.empty(self.shape, dtype=torch.float32, device=x.device)
+        elif out.dtype != torch.float32 or not out.is_cuda or not out.is_contiguous() or tuple(out.shape) != self.shape \
+                or out.device != x.device:
+            raise ValueError(f"FkSpectrum output must be a contiguous float32 CUDA tensor of shape {self.shape}")
+        nblocks = x.shape[1] // ns
+        L = _lib.lib()
+        with torch.cuda.device(self.device):
+            # x of exactly ns samples: x itself (through an aligned copy if it starts off the column kernels' boundary);
+            # otherwise each block is copied into one contiguous [nx, ns] buffer (one extra read and write of the block),
+            # and the power pass accumulates P / nblocks into out
+            whole = x.shape[1] == ns
+            if whole:
+                buf = x.clone() if _misaligned(x, ns) else x
+            else:
+                buf = torch.empty((nx, ns), dtype=x.dtype, device=x.device)
+            for b in range(nblocks):
+                if not whole:
+                    buf.copy_(x[:, b * ns:(b + 1) * ns])
+                _lib.check(L.d4w_fk_spectrum_apply(self.plan.ptr, self.ptr, _lib.ptr(buf, "float*"), _lib.ptr(out, "float*"),
+                                                   _lib.ptr(self._ws()), int(bool(tapering)), 1.0 / nblocks, int(b > 0),
+                                                   _lib.stream_ptr()), "fk_spectrum")
+        return out
