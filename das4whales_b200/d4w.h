@@ -160,6 +160,19 @@ size_t d4w_fk_spectrum_workspace_bytes(const d4w_fk_plan* plan, const d4w_fk_spe
 int    d4w_fk_spectrum_apply(d4w_fk_plan* plan, d4w_fk_spectrum* s, const float* dev_x, float* dev_out,
                              void* dev_workspace, int taper, float scale, int accumulate, void* stream);
 
+/* ---- f-k Welch spectrum: segment staging for d4w_fk_spectrum_apply -------------------------------------------- */
+/* Stage nseg segments of the float32 [nx x ns] matrix dev_x, all on channels [c0, c0 + lx): segment s (0 <= s < nseg)
+ * covers samples [t0 + s*step, t0 + s*step + l) and is written as a contiguous [lx x l] matrix at
+ * dev_out + s * seg_stride (floats):  out[s][c][t] = (x[c0 + c][t0 + s*step + t] - m) * wx[c] * wt[t],  m the mean of
+ * the row's l samples (accumulated in double) when detrend != 0, else 0.  dev_wx [lx] and dev_wt [l] are the channel and
+ * time windows.  dev_x is not modified.  D4W_ERR_ARG: a null pointer, segments outside the matrix, lx > 65 535,
+ * seg_stride < lx * l, dev_out / seg_stride that would leave a segment off the alignment d4w_fk_spectrum_apply needs
+ * for rows of l samples (16 bytes when l % 4 == 0, 8 when l is even), or a dev_wt that is not 16-byte aligned when
+ * l % 4 == 0. */
+int    d4w_fk_segment_stage(const float* dev_x, int nx, int ns, int c0, int lx, int t0, int l, int step, int nseg,
+                            const float* dev_wx, const float* dev_wt, int detrend, float* dev_out, size_t seg_stride,
+                            void* stream);
+
 /* ---- generic shared-memory FFT plan (matched-filter blocks, STFT frames) ----------------- */
 typedef struct d4w_fft_plan d4w_fft_plan;
 typedef struct d4w_row_plan d4w_row_plan;

@@ -330,11 +330,11 @@ def fk_filter_filts(trace, fk_filter_matrices, tapering=False):
     return [_to_host64(y) for y in ys]
 
 
-def _band(axis, lo, hi, what):
+def _band(axis, lo, hi, what, who="fk_spectrum"):
     """Half-open index range of {i : lo <= axis[i] <= hi} (a contiguous run: the shifted axes are monotonic)."""
     idx = np.flatnonzero((axis >= lo) & (axis <= hi))
     if idx.size == 0:
-        raise ValueError(f"fk_spectrum: {what} selects no bin of the axis [{axis[0]}, {axis[-1]}]")
+        raise ValueError(f"{who}: {what} selects no bin of the axis [{axis[0]}, {axis[-1]}]")
     return int(idx[0]), int(idx[-1]) + 1
 
 
@@ -377,6 +377,73 @@ def fk_spectrum(trace, selected_channels, dx, fs, f_range=(0., np.inf), k_range=
     p = spec(x, tapering=tapering)
     f, k = freq[f_idx[0]:f_idx[1]], knum[k_idx[0]:k_idx[1]]
     return (p if _is_tensor(trace) else _to_host64(p)), f, k
+
+
+fk_welch_layout = _fk.fk_welch_layout
+
+
+def fk_welch(trace, selected_channels, dx, fs, nperseg=None, noverlap=None, window="hann", nperseg_x=None, noverlap_x=None,
+             window_x="hann", detrend="constant", scaling="density", f_range=(0., np.inf), k_range=(-np.inf, np.inf)):
+    """f-k power spectral density by Welch's method, the 2-D (channel x time) counterpart of `welch`.
+
+    Time segments follow welch_layout (nperseg=None is 256, noverlap=None is nperseg // 2, a trailing partial segment is
+    dropped) and their spectra are averaged (mean).  Channel segments follow the same rules but are not averaged:
+    nperseg_x=None is one segment spanning every channel; with nperseg_x the result has a leading channel-segment axis.
+    window / window_x are resolved like welch_window (a string or tuple through scipy.signal.get_window, a 1-D array as
+    given, of length nperseg and nperseg_x or nx) and the 2-D window is their outer product.  detrend='constant' subtracts
+    each channel's mean over each segment before windowing; detrend=False does not.  The plane is two-sided, with
+    fsx = 1 / (selected_channels[2] * dx):  'density' is P / (fs fsx sum(wt^2) sum(wx^2)) in units^2 / Hz / (1/m),
+    'spectrum' is P / ((sum wt)^2 (sum wx)^2), P the mean of |fftshift(fft2(segment))|^2.  The axes are those of
+    fk_spectrum for the segment shape (freq = fftshift(fftfreq(nperseg, 1 / fs)), knum = fftshift(fftfreq(nperseg_x,
+    selected_channels[2] * dx))), cut to f_range and k_range with fk_spectrum's rules.
+
+    Returns (P, f, k) with P [len(k), len(f)], or (P, f, k, c0) with P [nseg_x, len(k), len(f)] and c0 the first channel
+    of each channel segment when nperseg_x is given.  An ndarray gives float64 ndarrays, a CUDA tensor a float32 CUDA P;
+    the caller's array is never modified.  ValueError for complex or non-2-D input, an empty or out-of-range segment
+    geometry, noverlap >= nperseg, a window of the wrong length, another detrend or scaling, and a segment shape the f-k
+    planner rejects (see supported_shape)."""
+    if _is_tensor(trace):
+        if trace.dim() != 2 or trace.is_complex():
+            raise ValueError(f"fk_welch: expected a real 2-D [channel x time] array, got {tuple(trace.shape)} {trace.dtype}")
+    else:
+        trace = np.asarray(trace)
+        if trace.ndim != 2 or np.iscomplexobj(trace):
+            raise ValueError(f"fk_welch: expected a real 2-D [channel x time] array, got {trace.shape} {trace.dtype}")
+    if detrend is not False and detrend != "constant":
+        raise ValueError(f"detrend={detrend!r}: only 'constant' and False are computed")
+    if scaling not in ("density", "spectrum"):
+        raise ValueError(f"Parameter scaling={scaling!r} not in {{'spectrum': 'magnitude', 'density': 'psd'}}!")
+    nx, ns = (int(v) for v in trace.shape)
+    if nx < 1 or ns < 1:
+        raise ValueError(f"fk_welch: empty record of shape {(nx, ns)}")
+    for what, n, lim in (("nperseg", nperseg, ns), ("nperseg_x", nperseg_x, nx)):
+        if n is not None and not 1 <= int(n) <= lim:
+            raise ValueError(f"fk_welch: {what} = {n} must lie in [1, {lim}]")
+    wt, lt = welch_window(window, nperseg, ns)
+    wx, lx = welch_window(window_x, nx if nperseg_x is None else nperseg_x, nx)
+    lay = fk_welch_layout(nx, ns, lt, noverlap, None if nperseg_x is None else lx, noverlap_x)
+    dxc = selected_channels[2] * dx
+    if scaling == "density":
+        scale = 1.0 / (fs * (1.0 / dxc) * float(np.sum(wt * wt)) * float(np.sum(wx * wx)))
+    else:
+        scale = 1.0 / (float(np.sum(wt)) ** 2 * float(np.sum(wx)) ** 2)
+    freq = np.fft.fftshift(np.fft.fftfreq(lt, 1 / fs))
+    knum = np.fft.fftshift(np.fft.fftfreq(lx, dxc))
+    f_idx = _band(freq, f_range[0], f_range[1], f"f_range {tuple(f_range)}", "fk_welch")
+    k_idx = _band(knum, k_range[0], k_range[1], f"k_range {tuple(k_range)}", "fk_welch")
+    x = _to_device(trace) if _is_tensor(trace) else None
+    device = x.device.index if x is not None else _fk._torch().cuda.current_device()
+    est = _fk.FkWelch((nx, ns), (lx, lt), k_idx, f_idx, wt, wx, detrend == "constant", scale, device=device,
+                      noverlap=lay.noverlap, noverlap_x=lay.noverlap_x)
+    if x is None:
+        x = _to_device(trace)
+    p = est(x)
+    f, k = freq[f_idx[0]:f_idx[1]], knum[k_idx[0]:k_idx[1]]
+    if not _is_tensor(trace):
+        p = _to_host64(p.reshape(-1, p.shape[-1])).reshape(tuple(p.shape))
+    if nperseg_x is None:
+        return p[0], f, k
+    return p, f, k, np.asarray(lay.starts_x, dtype=np.int64)
 
 
 # ------------------------------------------------------------------------------ IIR

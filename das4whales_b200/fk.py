@@ -1,13 +1,15 @@
 """Host side of the f-k filter: mask descriptors (`FkMask`), per-shape plans and the reusable
 `FkFilter` object that owns the device buffers.  dsp.fk_filter_design / hybrid_*_filter_design
 return `FkMask`; dsp.fk_filter_filt / fk_filter_sparsefilt run an `FkFilter`; dsp.fk_spectrum runs an
-`FkSpectrum` (the same forward transform, ending in |X|^2 over a band).
+`FkSpectrum` (the same forward transform, ending in |X|^2 over a band); dsp.fk_welch runs an `FkWelch`
+(staged, detrended and windowed segments through an FkSpectrum, averaged over time).
 
 All arithmetic happens in libd4w.so (hand-written sm_90a CUDA, see csrc/fk_kernels.cuh);
 PyTorch is used for device memory and streams only.
 """
 import threading
 import weakref
+from collections import namedtuple
 
 import numpy as np
 
@@ -542,4 +544,106 @@ class FkSpectrum:
                 _lib.check(L.d4w_fk_spectrum_apply(self.plan.ptr, self.ptr, _lib.ptr(buf, "float*"), _lib.ptr(out, "float*"),
                                                    _lib.ptr(self._ws()), int(bool(tapering)), 1.0 / nblocks, int(b > 0),
                                                    _lib.stream_ptr()), "fk_spectrum")
+        return out
+
+
+FkWelchLayout = namedtuple("FkWelchLayout", "nperseg noverlap step nseg starts nperseg_x noverlap_x step_x nseg_x starts_x")
+
+
+def fk_welch_layout(nx, ns, nperseg, noverlap, nperseg_x, noverlap_x):
+    """Segment geometry of the f-k Welch spectrum of an [nx, ns] record, pure Python (dsp.fk_welch's rules, those of
+    dsp.welch_layout on each axis).  nperseg=None is 256 and noverlap=None is nperseg // 2; time segment s covers samples
+    [starts[s], starts[s] + nperseg), starts[s] = s * step, step = nperseg - noverlap, nseg = (ns - nperseg) // step + 1
+    (a trailing partial segment is dropped).  The channel axis follows the same rules, except that nperseg_x=None is one
+    segment spanning all nx channels (noverlap_x is then ignored).  ValueError for an empty record, a segment length
+    outside [1, ns] (or [1, nx]) and an overlap that is not less than its segment length."""
+    nx, ns = int(nx), int(ns)
+    if nx < 1 or ns < 1:
+        raise ValueError(f"fk_welch: empty record of shape {(nx, ns)}")
+
+    def axis(n, nper, nover, what, default):
+        nper = default if nper is None else int(nper)
+        if not 1 <= nper <= n:
+            raise ValueError(f"fk_welch: {what} = {nper} must lie in [1, {n}]")
+        nover = nper // 2 if nover is None else int(nover)
+        if nover >= nper:
+            raise ValueError(f"fk_welch: the overlap {nover} must be less than {what} = {nper}")
+        step = nper - nover
+        nseg = (n - nper) // step + 1
+        return nper, nover, step, nseg, tuple(s * step for s in range(nseg))
+
+    t = axis(ns, nperseg, noverlap, "nperseg", 256)
+    c = axis(nx, nperseg_x, noverlap_x if nperseg_x is not None else 0, "nperseg_x", nx)
+    return FkWelchLayout(*t, *c)
+
+
+# staging buffer of FkWelch: as many whole segments as fit this many bytes, at least one
+FK_WELCH_STAGE_BYTES = 512 << 20
+
+
+class FkWelch:
+    """f-k power spectral density by Welch's method over one record shape (dsp.fk_welch): segments of segment_shape
+    (Lx, L) are detrended, windowed and staged as contiguous matrices (d4w_fk_segment_stage), each goes through an
+    FkSpectrum of that shape, and the power pass averages the time segments of one channel segment in place.
+
+    >>> w = FkWelch((nx, ns), (Lx, L), (k0, k1), (f0, f1), wt, wx, True, scale, device=0, noverlap=L // 2)
+    >>> p = w(x_cuda)          # float32 [nseg_x, k1 - k0, f1 - f0]: scale * the mean over time segments, per channel segment
+
+    window (L) and window_x (Lx) are float arrays; scale multiplies the mean periodogram (dsp.fk_welch passes the density
+    or spectrum normalisation).  noverlap / noverlap_x follow fk_welch_layout; with Lx == nx there is one channel segment.
+    `layout` is the fk_welch_layout, `batch` the number of time segments staged per launch (FK_WELCH_STAGE_BYTES)."""
+
+    def __init__(self, shape, segment_shape, k_idx, f_idx, window, window_x, detrend, scale, device=None, noverlap=None,
+                 noverlap_x=None):
+        torch = _torch()
+        nx, ns = int(shape[0]), int(shape[1])
+        lx, l = int(segment_shape[0]), int(segment_shape[1])
+        self.layout = fk_welch_layout(nx, ns, l, noverlap, lx, noverlap_x)
+        wt, wx = np.asarray(window, dtype=np.float64), np.asarray(window_x, dtype=np.float64)
+        if wt.shape != (l,) or wx.shape != (lx,):
+            raise ValueError(f"FkWelch: windows of shapes {wt.shape} and {wx.shape} for segments of {(lx, l)} "
+                             f"(time window [{l}], channel window [{lx}])")
+        self.shape, self.segment_shape = (nx, ns), (lx, l)
+        self.spec = FkSpectrum((lx, l), k_idx, f_idx, device=device)
+        self.device, self.plan = self.spec.device, self.spec.plan
+        self.detrend, self.scale = bool(detrend), float(scale)
+        self.out_shape = (self.layout.nseg_x,) + self.spec.shape
+        dev = f"cuda:{self.device}"
+        self.wt = torch.from_numpy(wt).to(dev, torch.float32)
+        self.wx = torch.from_numpy(wx).to(dev, torch.float32)
+        # each staged segment starts 16 bytes aligned: the column kernels' boundary for rows of L samples
+        self.seg_stride = (lx * l + 3) // 4 * 4
+        self.batch = max(1, min(self.layout.nseg, FK_WELCH_STAGE_BYTES // (4 * self.seg_stride)))
+        self.buf = torch.empty(self.batch * self.seg_stride, dtype=torch.float32, device=dev)
+
+    def __call__(self, x, out=None):
+        """P [nseg_x, k1 - k0, f1 - f0] of x [nx, ns] (contiguous float32 CUDA); x is never modified."""
+        torch = _torch()
+        if x.dtype != torch.float32 or not x.is_cuda or not x.is_contiguous() or x.dim() != 2:
+            raise ValueError("FkWelch expects a contiguous 2-D float32 CUDA tensor")
+        if tuple(x.shape) != self.shape:
+            raise ValueError(f"FkWelch built for records of {self.shape}, got {tuple(x.shape)}")
+        if out is None:
+            out = torch.empty(self.out_shape, dtype=torch.float32, device=x.device)
+        elif out.dtype != torch.float32 or not out.is_cuda or not out.is_contiguous() or tuple(out.shape) != self.out_shape \
+                or out.device != x.device:
+            raise ValueError(f"FkWelch output must be a contiguous float32 CUDA tensor of shape {self.out_shape}")
+        lay, (nx, ns), (lx, l) = self.layout, self.shape, self.segment_shape
+        L = _lib.lib()
+        plane = self.spec.shape[0] * self.spec.shape[1]
+        scale = self.scale / lay.nseg
+        with torch.cuda.device(self.device):
+            ws = _lib.ptr(self.spec._ws())
+            stream = _lib.stream_ptr()
+            for j, c0 in enumerate(lay.starts_x):
+                dst = _lib.ffi.cast("float*", out.data_ptr() + 4 * j * plane)
+                for s0 in range(0, lay.nseg, self.batch):
+                    cnt = min(self.batch, lay.nseg - s0)
+                    _lib.check(L.d4w_fk_segment_stage(_lib.ptr(x, "float*"), nx, ns, c0, lx, lay.starts[s0], l, lay.step, cnt,
+                                                      _lib.ptr(self.wx, "float*"), _lib.ptr(self.wt, "float*"), int(self.detrend),
+                                                      _lib.ptr(self.buf, "float*"), self.seg_stride, stream), "fk_welch stage")
+                    for s in range(cnt):
+                        seg = _lib.ffi.cast("float*", self.buf.data_ptr() + 4 * s * self.seg_stride)
+                        _lib.check(L.d4w_fk_spectrum_apply(self.plan.ptr, self.spec.ptr, seg, dst, ws, 0, scale,
+                                                           int(s0 + s > 0), stream), "fk_welch")
         return out
