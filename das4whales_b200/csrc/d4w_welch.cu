@@ -3,12 +3,10 @@
 // welch_kernels.cuh; a median over more segments than fit shared memory goes through the workspace and d4w_row_median.
 // Its own translation unit, so the kernels of d4w_rows.cu keep their code.
 #include <climits>
-#include <map>
-#include <mutex>
 #include <string>
 #include "d4w_common.hpp"
 #include "welch_kernels.cuh"
-#include "xcorr_launch.cuh"
+#include "plan_k2pos.cuh"
 
 using namespace d4w;
 
@@ -37,26 +35,6 @@ int welch_max_nfft(size_t cap) {
     int n = 2;
     while (welch_smem_bytes(n + 1, (n + 1) / 2 + 1, 1, 1, kWelchMean) <= cap) ++n;
     return n;
-}
-
-// Bin -> position map of the stages k_welch runs (p->pl).  The plan's d_k2pos inverts its pos2k, which for the prime-factor
-// length (p->pfa, n = 2520) is the matched filter's Good-Thomas map, not the map of p->pl: for that length a table of
-// p->pl's own map is built once per device and kept for the life of the process (one 10 KB table per device).
-cudaError_t welch_k2pos(const d4w_fft_plan* p, const int** out) {
-    if (!p->pfa) { *out = p->d_k2pos; return cudaSuccess; }
-    static std::mutex mu;
-    static std::map<int, int*> tables;
-    std::lock_guard<std::mutex> lock(mu);
-    int*& t = tables[p->device];
-    if (!t) {
-        const std::vector<int> p2k = make_pos2freq(p->pl);
-        std::vector<int> k2pos(p2k.size());
-        for (size_t i = 0; i < p2k.size(); ++i) k2pos[p2k[i]] = (int)i;
-        const cudaError_t e = upload(&t, k2pos);
-        if (e != cudaSuccess) { cudaFree(t); t = nullptr; return e; }
-    }
-    *out = t;
-    return cudaSuccess;
 }
 
 }  // namespace

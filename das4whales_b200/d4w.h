@@ -276,6 +276,27 @@ int d4w_welch(d4w_fft_plan* plan, const float* dev_x, int nrows, int ns, int chu
               const float* dev_window, int detrend, double scale, int average, float* dev_out, void* dev_workspace,
               void* stream);
 
+/* ---- cross-spectral density and coherence of row pairs: scipy.signal.csd(x, y, fs, window, nperseg, noverlap, nfft,
+ *      detrend, return_onesided=True, scaling, average) and scipy.signal.coherence(x, y, ...) for every output row at once.
+ *      Output row r pairs the ns samples at dev_x + r * x_row_stride with those at dev_y + r * y_row_stride (floats); a
+ *      stride of 0 broadcasts one row against every row of the other side (the neighbour pairs x[:-1], x[1:] of a
+ *      contiguous matrix are dev_x, dev_x + ns with both strides ns).  Segments, detrending, window, nfft = the plan's
+ *      length and scale are d4w_welch's (with chunk = ns).  Per segment P_k = conj(X_k) Y_k * scale, doubled at every bin
+ *      but DC and, for even nfft, Nyquist.
+ *      what 0: Pxy, dev_out float2 [nrows][nfft / 2 + 1], averaged over the segments: average 0 = mean, 1 = (np.median of
+ *      Re + i np.median of Im) / _median_bias(nseg).
+ *      what 1: Cxy = |Pxy|^2 / (Pxx Pyy) of the mean spectra (average must be 0), dev_out float [nrows][nfft / 2 + 1]; a
+ *      row whose Pxx or Pyy is 0 gives NaN, as 0 / 0 in NumPy.
+ *      Every nfft the plan accepts whose one complex frame plus the bin sums of the mean route (2 doubles per bin for Pxy, 4
+ *      for Cxy; the workspace median keeps none) fits shared memory: D4W_ERR_UNSUPPORTED names the limit of the route taken.  D4W_ERR_ARG: nrows < 1, nperseg outside [1, ns], step < 1,
+ *      nfft < nperseg, a row stride neither 0 nor >= ns, what = 1 with average = 1.
+ *      dev_workspace: d4w_csd_workspace_bytes bytes (0 unless a median over more segments than fit shared memory, which
+ *      writes every periodogram as [nrows][nbins][re, im][nseg] floats and selects each row of nseg signed values). */
+size_t d4w_csd_workspace_bytes(const d4w_fft_plan* plan, int nrows, int ns, int nperseg, int step, int what, int average);
+int d4w_csd(d4w_fft_plan* plan, const float* dev_x, long long x_row_stride, const float* dev_y, long long y_row_stride,
+            int nrows, int ns, int nperseg, int step, const float* dev_window, int detrend, double scale, int what,
+            int average, void* dev_out, void* dev_workspace, void* stream);
+
 /* ---- spectrogram-correlation detector: detect.xcorr2d / compute_cross_correlogram_spectrocorr
  *      (detect.py:579-602, :650-708).  Per-row median / maximum of a float32 matrix [nrows][n]
  *      (entries must be >= 0 for the median), and

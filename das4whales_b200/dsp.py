@@ -631,6 +631,76 @@ def welch(x, fs=1.0, window="hann_periodic", nperseg=None, noverlap=None, nfft=N
     return f, (p if tensor else _to_host64(p))
 
 
+def _cross_spectrum(name, x, y, fs, window, nperseg, noverlap, nfft, detrend, return_onesided, scaling, axis, average,
+                    coherence):
+    """csd / coherence: every check before any device work, then one rows.csd over all row pairs"""
+    tensor = _is_tensor(x) or _is_tensor(y)
+    a = x if _is_tensor(x) else np.asarray(x)
+    b = y if _is_tensor(y) else np.asarray(y)
+    for v in (a, b):
+        if v.ndim not in (1, 2):
+            raise ValueError(f"{name} takes 1-D or 2-D input, not {v.ndim}-D")
+        if int(axis) not in (-1, v.ndim - 1):
+            raise ValueError(f"{name} computes along the last axis only (axis=-1)")
+        if (v.is_complex() if _is_tensor(v) else np.iscomplexobj(v)):
+            raise ValueError(f"{name} takes real input only")
+    ns = int(a.shape[-1])
+    if int(b.shape[-1]) != ns:
+        raise ValueError(f"{name}: x and y must have the same length, not {ns} and {int(b.shape[-1])} (zero-padding the "
+                         "shorter one is not computed)")
+    nx, ny = (int(v.shape[0]) if v.ndim == 2 else 1 for v in (a, b))
+    if nx != ny and 1 not in (nx, ny):
+        raise ValueError(f"{name}: x and y cannot be broadcast together ({nx} and {ny} rows)")
+    if not return_onesided:
+        raise ValueError(f"{name} computes one-sided spectra only (return_onesided=True)")
+    if detrend is not False and detrend != "constant":
+        raise ValueError(f"detrend={detrend!r}: only 'constant' and False are computed")
+    if average not in ("mean", "median"):
+        raise ValueError(f"Parameter average={average!r} must be 'median' or 'mean'!")
+    win, nperseg = welch_window(window, nperseg, ns)
+    lay = welch_layout(ns, nperseg, noverlap, nfft)
+    scale = welch_scale(win, fs, scaling)
+    cuda = [v.device for v in (a, b) if _is_tensor(v) and v.is_cuda]
+    with _fk._torch().cuda.device(cuda[0] if cuda else None):        # an ndarray joins the tensor on its device
+        xd = _to_device(a)
+        yd = xd if y is x else _to_device(b)
+    xd, yd = xd.reshape(-1, ns), yd.reshape(-1, ns)
+    p = _rows.csd(xd, yd, lay.nperseg, lay.step, lay.nfft, win, detrend == "constant", scale, average, coherence)
+    f = np.fft.rfftfreq(lay.nfft, 1 / fs)
+    if a.ndim == 1 and b.ndim == 1:
+        p = p[0]
+    if tensor:
+        return f, p
+    if coherence:
+        return f, _to_host64(p)
+    h = np.ascontiguousarray(_to_host64(_fk._torch().view_as_real(p)))
+    return f, h.view(np.complex128)[..., 0]
+
+
+def csd(x, y, fs=1.0, window="hann_periodic", nperseg=None, noverlap=None, nfft=None, detrend="constant",
+        return_onesided=True, scaling="density", axis=-1, average="mean"):
+    """scipy.signal.csd (SciPy 1.18 defaults) of 1-D or 2-D real input along the last axis, every row pair in one d4w_csd
+    call.  x and y have the same length and the same number of rows, or one of them is a single row (1-D or [1, ns]) that
+    is paired with every row of the other; x[:-1], x[1:] are the neighbour pairs.  Returns (f, Pxy): f = rfftfreq(nfft,
+    1 / fs) as a float64 ndarray; Pxy [nbins] (both 1-D) or [max(rows), nbins], Pxy = conj(X) Y averaged over the segments,
+    a complex128 ndarray for ndarrays in and a complex64 CUDA tensor when either input is a tensor.  y is x gives the real
+    dsp.welch(x), as SciPy returns the real part.  ValueError, with no fall-back to SciPy, for what the kernel does not
+    compute: unequal lengths, detrend other than 'constant' or False, return_onesided=False, another axis, complex input."""
+    if y is x:
+        return welch(x, fs, window, nperseg, noverlap, nfft, detrend, return_onesided, scaling, axis, average)
+    return _cross_spectrum("csd", x, y, fs, window, nperseg, noverlap, nfft, detrend, return_onesided, scaling, axis, average,
+                           False)
+
+
+def coherence(x, y, fs=1.0, window="hann_periodic", nperseg=None, noverlap=None, nfft=None, detrend="constant", axis=-1):
+    """scipy.signal.coherence (SciPy 1.18 defaults): Cxy = |Pxy|^2 / (Pxx Pyy) of the mean Welch spectra, with csd's
+    shapes, pairing and errors; one d4w_csd call computes all three spectra of every row pair.  Returns (f, Cxy): Cxy a
+    float64 ndarray for ndarrays in and a float32 CUDA tensor when either input is a tensor.  A row of zeros gives NaN, as
+    0 / 0 does in NumPy.  coherence(trace[:-1], trace[1:]) is the neighbour-channel coherence along a cable."""
+    return _cross_spectrum("coherence", x, y, fs, window, nperseg, noverlap, nfft, detrend, True, "density", axis, "mean",
+                           True)
+
+
 # ------------------------------------------------------------------------------ cable noise profile
 NOISE_PROFILE_KEYS = ("med", "mean", "std", "std_med_diff", "SNR_1d", "noise_power", "noise_power_db", "noise_mean")
 

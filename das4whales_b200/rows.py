@@ -442,6 +442,53 @@ def welch(x, nperseg, step, nfft, window, detrend, scale, average, chunk=None):
     return out
 
 
+def csd(x, y, nperseg, step, nfft, window, detrend, scale, average, coherence=False):
+    """Cross-spectral density or coherence of row pairs (d4w_csd), on the Welch geometry of rows.welch (whole rows): x, y
+    contiguous float32 CUDA [rows, ns] on one device with equal row counts, or one of them a single row, which is paired
+    with every row of the other.  Pxy = conj(X) Y averaged by 'mean' or 'median'; coherence=True gives
+    |Pxy|^2 / (Pxx Pyy) of the mean spectra.  Returns complex64 (Pxy) or float32 (Cxy) CUDA [max(rows), nfft // 2 + 1]."""
+    torch = _torch()
+    dev = _check_input(x)
+    if _check_input(y) != dev:
+        raise ValueError("csd: x and y must be on the same device")
+    (nx, ns), (ny, nsy) = x.shape, y.shape
+    if ns != nsy:
+        raise ValueError(f"csd: x and y must have the same length, not {ns} and {nsy}")
+    if nx != ny and 1 not in (nx, ny):
+        raise ValueError(f"csd: {nx} rows of x and {ny} rows of y cannot be broadcast together")
+    if average not in ("mean", "median"):
+        raise ValueError(f"average must be 'mean' or 'median', not {average!r}")
+    if coherence and average != "mean":
+        raise ValueError("the coherence is computed from mean spectra only")
+    med, what = (1 if average == "median" else 0), (1 if coherence else 0)
+    plan = fft_plan(int(nfft), dev)
+    win = np.ascontiguousarray(window, dtype=np.float32)
+    if win.shape != (int(nperseg),):
+        raise ValueError(f"window of shape {win.shape} for segments of {nperseg} samples")
+    wd = torch.from_numpy(win).to(x.device)
+    nrows, nbins = (0 if 0 in (nx, ny) else max(nx, ny)), int(nfft) // 2 + 1        # 0 rows broadcast to 0, as in NumPy
+    out = torch.empty((nrows, nbins) if coherence else (nrows, nbins, 2), dtype=torch.float32, device=x.device)
+    if nrows == 0:
+        return out if coherence else torch.view_as_complex(out)
+    L = _lib.lib()
+    args = (ns, int(nperseg), int(step), what, med)
+    per_row = int(L.d4w_csd_workspace_bytes(plan.ptr, 1, *args))
+    max_rows = nrows if per_row == 0 else max(1, min(nrows, _WELCH_WS_ROWS_BYTES // per_row))
+    with torch.cuda.device(dev):
+        ws = torch.empty(max(1, per_row * max_rows), dtype=torch.uint8, device=x.device)
+        for r0 in range(0, nrows, max_rows):
+            r1 = min(nrows, r0 + max_rows)
+            xp, xs = (x[0], 0) if nx == 1 else (x[r0], ns)
+            yp, ys = (y[0], 0) if ny == 1 else (y[r0], ns)
+            rc = L.d4w_csd(plan.ptr, _lib.ptr(xp, "float*"), xs, _lib.ptr(yp, "float*"), ys, r1 - r0, ns, int(nperseg),
+                           int(step), _lib.ptr(wd, "float*"), 1 if detrend else 0, float(scale), what, med,
+                           _lib.ptr(out[r0:r1]), _lib.ptr(ws), _lib.stream_ptr())
+            if rc == 2:             # D4W_ERR_UNSUPPORTED: the nfft limit, named in the message
+                raise ValueError("csd: " + _lib.ffi.string(L.d4w_last_error()).decode(errors="replace"))
+            _lib.check(rc, "csd")
+    return out if coherence else torch.view_as_complex(out)
+
+
 # ------------------------------------------------------------------------------ spectrogram correlation
 def row_max(x2d):
     """max over the last axis of a [rows, n] float32 CUDA tensor"""
