@@ -373,6 +373,31 @@ int d4w_loc_grid(const double* dev_T, const double* dev_pos, const long long* de
 int d4w_loc_solve(const double* dev_T, const double* dev_pos, const long long* dev_offsets, int ncalls, double c0, int nbiter,
                   int fix_z, const double* dev_n0, double* dev_n, double* dev_var, double* dev_unc, double* dev_cinv,
                   double* dev_cond, double* dev_traj, double* dev_n0_used, void* stream);
+/* ---- pick association by back-projection over a source grid, in FP64 (loc.associate_picks).  Picks are a CSR by channel:
+ *      channel c (c < n_channels, at dev_cable_pos[c][3], m) holds the int32 samples dev_samples[dev_offsets[c] ..
+ *      dev_offsets[c + 1]), n_picks = dev_offsets[n_channels]; the pipelines' (offsets, idx).  Nodes as d4w_loc_grid.
+ *      T_p = s_p / fs; tau(g, c) = sqrt(dx dx + dy dy + dz dz) / c0, dx = cable_pos[c][0] - g_x (likewise y, z), left to right,
+ *      every operation rounded on its own (no fused multiply-add); o = T_p - tau; bin j = floor(o r) with h = tol / 2 and
+ *      r = 1 / h given by the caller.  n(g, j) counts the unassigned picks in bin j of node g; (g, j) scores n(g, j) + n(g, j + 1).
+ *      Repeated: the (g, j) of highest score, ties to the lowest node, then the lowest j; stop when the score is below
+ *      min_picks or after max_calls calls; else call k gets dev_node[k] = g, dev_t0[k] = (j + 1) h, the unassigned picks with
+ *      bin j or j + 1 (dev_labels[p] = k, int64, CSR order; -1 for a pick of no call) and dev_count[k] = their number.
+ *      *n_calls = K.  Two picks of one channel count separately; a straight cable cannot tell a source from its mirror
+ *      image, and the tie rule then returns the lower node index.  Deterministic: integer counts, fixed reduction order.
+ *  d4w_loc_assoc_bins: the bin range [*jlo, *jlo + *nbins) that covers every origin time of picks with T in [t_min, t_max]
+ *      at channels inside host_box[0..5] = (min x, y, z, max x, y, z) from nodes inside host_box[6..11] (host memory, no
+ *      device work).  D4W_ERR_UNSUPPORTED, naming the limit, when the vote's histogram (4 nodes x (nbins + 1) ints per
+ *      block) does not fit shared memory: raise tol or shorten the record.  d4w_loc_associate applies it to the picks' own
+ *      range (one small read-back), and reads back one record per extracted call; no per-pick data leaves the device.
+ *      D4W_ERR_ARG: offsets that do not rise from 0 to n_picks, a negative sample.  dev_workspace:
+ *      d4w_loc_assoc_workspace_bytes bytes. */
+int d4w_loc_assoc_bins(double t_min, double t_max, const double* host_box, double c0, double r, long long* jlo, int* nbins);
+size_t d4w_loc_assoc_workspace_bytes(long long n_picks, int nx, int ny, int nz);
+int d4w_loc_associate(const int* dev_offsets, const int* dev_samples, int n_channels, long long n_picks, double fs,
+                      const double* dev_cable_pos, double c0, const double* dev_gx, int nx, const double* dev_gy, int ny,
+                      const double* dev_gz, int nz, double h, double r, int min_picks, int max_calls, void* dev_workspace,
+                      long long* dev_labels, long long* dev_node, double* dev_t0, long long* dev_count, int* n_calls,
+                      void* stream);
 
 /* ---- image operators of improcess outside the Gabor path (das4whales/improcess.py:143-169, :319-367).
  *  d4w_radon: skimage.transform.radon(image, theta, circle=False) of the float32 image [h][w] placed at rows

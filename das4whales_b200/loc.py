@@ -3,7 +3,9 @@
 The geometry helpers and `cal_variance_residuals` are host NumPy, as in the reference.  `solve_lq`,
 `calc_covariance_matrix` and `calc_uncertainty_position` keep the reference's signatures and run on the GPU
 (d4w_loc_solve); `solve_lq_batch` solves many calls in one launch, optionally from the best node of a grid search
-(d4w_loc_grid), and `localize_picks` solves the calls of a pick list cut by time windows.  Everything is float64.
+(d4w_loc_grid), and `localize_picks` solves the calls of a pick list cut by time windows.  `associate_picks` groups a
+file's picks into calls by back-projection over a source grid (d4w_loc_associate), and `localize_calls` solves every call
+it finds, so no time window is needed.  Everything is float64.
 """
 import sys
 from collections import namedtuple
@@ -242,6 +244,196 @@ def localize_picks(idx_tp, fs, windows, cable_pos, c0, Nbiter=10, fix_z=False, g
     solve_lq_batch, whose Localisation (ndarrays) is returned."""
     T, pos, offsets = picks_to_batch(idx_tp, fs, windows, cable_pos)
     return solve_lq_batch(T, pos, offsets, c0, Nbiter=Nbiter, fix_z=fix_z, grid=grid)
+
+
+# ------------------------------------------------------------------------------ association of picks into calls
+Association = namedtuple("Association", "labels node t0 count")
+Association.__doc__ = """Result of associate_picks for K calls: labels [n_picks] int64, the call of each pick or -1; node [K] int64,
+the grid node index of each call; t0 [K] float64, its origin time (s); count [K] int64, its number of picks.  Calls are
+numbered in extraction order (highest score first)."""
+
+
+def _assoc_picks(picks, ncable):
+    """('device', offsets int32, samples int32) or ('host', ch int64, s int64), validated"""
+    if isinstance(picks, (tuple, list)) and len(picks) == 2 and all(_is_tensor(a) for a in picks):
+        import torch
+        offsets, idx = picks
+        if not (offsets.is_cuda and idx.is_cuda and offsets.dtype == torch.int32 and idx.dtype == torch.int32
+                and offsets.ndim == 1 and idx.ndim == 1 and offsets.numel() >= 2):
+            raise ValueError("device picks must be (offsets int32 [n_channels + 1], idx int32 [n_picks]) CUDA tensors")
+        if offsets.numel() - 1 > ncable:
+            raise ValueError(f"a picked channel is outside cable_pos: the picks have {offsets.numel() - 1} channels, "
+                             f"cable_pos {ncable} rows")
+        return "device", offsets.contiguous(), idx.contiguous()
+    try:
+        a = np.asarray(picks)
+    except (TypeError, ValueError):
+        raise ValueError("picks must be [[channel ...], [sample ...]] or the device (offsets, idx)") from None
+    if a.ndim != 2 or a.shape[0] != 2 or not (a.size == 0 or np.issubdtype(a.dtype, np.integer)):
+        raise ValueError("picks must be [[channel ...], [sample ...]] of integers or the device (offsets, idx)")
+    ch, s = a[0].astype(np.int64), a[1].astype(np.int64)
+    if ch.size and (ch.min() < 0 or ch.max() >= ncable):
+        raise ValueError("a picked channel is outside cable_pos")
+    if s.size and s.min() < 0:
+        raise ValueError("a pick has a negative sample")
+    if s.size and s.max() > np.iinfo(np.int32).max:
+        raise ValueError("pick samples must be below 2**31")
+    return "host", ch, s
+
+
+def _assoc_check(picks, fs, cable_pos, c0, grid, tol, min_picks, max_calls):
+    for name, v in (("fs", fs), ("c0", c0), ("tol", tol)):
+        if not (isinstance(v, (int, float, np.integer, np.floating)) and np.isfinite(v) and v > 0):
+            raise ValueError(f"{name} must be positive and finite")
+    for name, v in (("min_picks", min_picks), ("max_calls", max_calls)):
+        if int(v) != v or v < 1:
+            raise ValueError(f"{name} must be an integer >= 1")
+    axes = _grid_axes(grid, False)
+    if not all(np.all(np.isfinite(a)) for a in axes):
+        raise ValueError("grid bounds must be finite")
+    cable_pos = np.asarray(cable_pos.cpu() if _is_tensor(cable_pos) else cable_pos, dtype=np.float64)
+    if cable_pos.ndim != 2 or cable_pos.shape[1] != 3 or cable_pos.shape[0] == 0 or not np.all(np.isfinite(cable_pos)):
+        raise ValueError(f"cable_pos must be finite [channels, 3], got {cable_pos.shape}")
+    kind, a, b = _assoc_picks(picks, cable_pos.shape[0])
+    h = float(tol) / 2.0
+    r = 1.0 / h
+    if kind == "host" and a.size:
+        # the histogram bound the device applies to the picks' range, checked here before any device work
+        used = cable_pos[np.unique(a)]
+        box = np.r_[used.min(0), used.max(0), [x.min() for x in axes], [x.max() for x in axes]]
+        _assoc_bins(b.min() / float(fs), b.max() / float(fs), box, float(c0), r)
+    return kind, a, b, cable_pos, axes, h, r
+
+
+def _assoc_bins(tmin, tmax, box, c0, r):
+    L = _lib.lib()
+    box = np.ascontiguousarray(box, dtype=np.float64)
+    jlo, nb = _lib.ffi.new("long long*"), _lib.ffi.new("int*")
+    rc = L.d4w_loc_assoc_bins(float(tmin), float(tmax), _lib.ffi.cast("double*", box.ctypes.data), c0, r, jlo, nb)
+    _assoc_rc(rc)
+
+
+def _assoc_rc(rc):
+    if rc == 2:           # D4W_ERR_UNSUPPORTED: the vote's histogram does not fit shared memory
+        msg = _lib.ffi.string(_lib.lib().d4w_last_error()).decode(errors="replace")
+        raise ValueError(f"associate_picks: {msg}: raise tol or shorten the record")
+    _lib.check(rc, "loc_associate")
+
+
+def _associate_device(offsets, samples, fs, cable_pos, c0, axes, h, r, min_picks, max_calls):
+    """device CSR in, (labels, node, t0, count) CUDA tensors out (labels in CSR order)"""
+    torch = _torch()
+    L = _lib.lib()
+    dev = offsets.device
+    nch, npk = offsets.numel() - 1, samples.numel()
+    P = _dev(cable_pos, dev)
+    gx, gy, gz = (_dev(a, dev) for a in axes)
+    ws = torch.empty(max(1, int(L.d4w_loc_assoc_workspace_bytes(npk, gx.numel(), gy.numel(), gz.numel()))),
+                     dtype=torch.uint8, device=dev)
+    labels = torch.empty(npk, dtype=torch.int64, device=dev)
+    node = torch.empty(max_calls, dtype=torch.int64, device=dev)
+    t0 = torch.empty(max_calls, dtype=torch.float64, device=dev)
+    count = torch.empty(max_calls, dtype=torch.int64, device=dev)
+    K = _lib.ffi.new("int*")
+    _assoc_rc(L.d4w_loc_associate(_lib.ptr(offsets, "int*"), _lib.ptr(samples, "int*"), nch, npk, float(fs), _pd(P),
+                                  float(c0), _pd(gx), gx.numel(), _pd(gy), gy.numel(), _pd(gz), gz.numel(), h, r,
+                                  int(min_picks), int(max_calls), _lib.ptr(ws), _lib.ptr(labels, "long long*"),
+                                  _lib.ptr(node, "long long*"), _pd(t0), _lib.ptr(count, "long long*"), K,
+                                  _lib.stream_ptr()))
+    k = int(K[0])
+    return Association(labels, node[:k], t0[:k], count[:k])
+
+
+def _host_csr(ch, s, ncable, dev):
+    """host picks -> (order, device offsets int32, device samples int32) in channel-major, stable order"""
+    torch = _torch()
+    order = np.argsort(ch, kind="stable")
+    off = np.zeros(ncable + 1, dtype=np.int32)
+    off[1:] = np.cumsum(np.bincount(ch, minlength=ncable))
+    return order, _dev(off, dev), _dev(s[order].astype(np.int32), dev)
+
+
+def associate_picks(picks, fs, cable_pos, c0, grid, tol, min_picks, max_calls=64):
+    """Group picks into calls by back-projection over a source grid, on the GPU.
+
+    picks: the host [[channel ...], [sample ...]] of detect.convert_pick_times / picks_to_host, or the device
+    (offsets, idx) of a pipeline's process_device.  cable_pos [n_channels, 3] (m), row c = channel c; c0 the sound speed;
+    grid = ((x0, x1, nx), (y0, y1, ny), (z0, z1, nz)) as grid_search.  For every node g each pick implies an origin time
+    T - |pos - g| / c0, binned on a grid of step tol / 2; a call is the node and window of width tol (two adjacent bins)
+    holding the most unassigned picks, taken while it holds at least min_picks, at most max_calls times.  The exact rule
+    is d4w_loc_associate's (include/d4w.h).  Two picks of one channel count separately.  A straight cable cannot tell a
+    source from its mirror image: the lower node index wins, so restrict the grid to one side of the cable.
+
+    Returns an Association.  Host picks give ndarrays with labels in the given order; device picks give CUDA tensors
+    with labels in CSR order (picks_to_host's order).  ValueError for bad arguments, and when the origin times span more
+    bins than fit shared memory (raise tol or shorten the record)."""
+    kind, a, b, cable_pos, axes, h, r = _assoc_check(picks, fs, cable_pos, c0, grid, tol, min_picks, max_calls)
+    torch = _torch()
+    if kind == "device":
+        with torch.cuda.device(a.device):
+            return _associate_device(a, b, fs, cable_pos, c0, axes, h, r, min_picks, max_calls)
+    dev = _device_of(False, None)
+    with torch.cuda.device(dev):
+        order, offd, sd = _host_csr(a, b, cable_pos.shape[0], dev)
+        res = _associate_device(offd, sd, fs, cable_pos, c0, axes, h, r, min_picks, max_calls)
+        lab_csr = res.labels.cpu().numpy()
+    labels = np.empty_like(lab_csr)
+    labels[order] = lab_csr
+    return Association(labels, res.node.cpu().numpy(), res.t0.cpu().numpy(), res.count.cpu().numpy())
+
+
+def localize_calls(picks, fs, cable_pos, c0, grid, tol, min_picks, max_calls=64, Nbiter=10, fix_z=False):
+    """associate_picks, then one solve_lq_batch over the calls: call k's observations are its picks in CSR order
+    (channel, then pick order within the channel), T = sample / fs at cable_pos[channel], from the first guess
+    n0 = (node x, y, z, t0).  fix_z needs nz = 1.  Returns (Association, Localisation), both ndarrays for host picks and
+    CUDA tensors for device picks; with no call the Localisation has 0 rows."""
+    if fix_z:
+        _grid_axes(grid, True)
+    kind, a, b, cable_pos, axes, h, r = _assoc_check(picks, fs, cable_pos, c0, grid, tol, min_picks, max_calls)
+    torch = _torch()
+    dev = a.device if kind == "device" else _device_of(False, None)
+    with torch.cuda.device(dev):
+        if kind == "device":
+            offd, sd = a, b
+        else:
+            order, offd, sd = _host_csr(a, b, cable_pos.shape[0], dev)
+        res = _associate_device(offd, sd, fs, cable_pos, c0, axes, h, r, min_picks, max_calls)
+        T, pos, off, n0 = _calls_batch(res, offd, sd, fs, cable_pos, axes, dev)
+        K = res.node.numel()
+        if K:
+            loc_ = solve_lq_batch(T, pos, off, c0, Nbiter=Nbiter, fix_z=fix_z, n0=n0)
+        else:
+            p = 3 if fix_z else 4
+            z = lambda *s: torch.empty(s, dtype=torch.float64, device=dev)     # noqa: E731
+            loc_ = Localisation(z(0, 4), z(0), z(0, p), torch.empty(0, dtype=torch.int64, device=dev), z(0, 4))
+    if kind == "device":
+        return res, loc_
+    labels = np.empty(res.labels.numel(), dtype=np.int64)
+    labels[order] = res.labels.cpu().numpy()
+    assoc = Association(labels, res.node.cpu().numpy(), res.t0.cpu().numpy(), res.count.cpu().numpy())
+    return assoc, Localisation(*(t.cpu().numpy() for t in loc_))
+
+
+def _calls_batch(res, offd, sd, fs, cable_pos, axes, dev):
+    """(T, pos, offsets, n0) of solve_lq_batch for the calls of an association, gathered on the device: call k's picks in
+    CSR order, its first guess (node, t0)"""
+    torch = _torch()
+    K = res.node.numel()
+    nch = offd.numel() - 1
+    ch = torch.repeat_interleave(torch.arange(nch, device=dev), (offd[1:] - offd[:-1]).long())
+    lab = res.labels
+    keep = torch.nonzero(lab >= 0).flatten()
+    rows = keep[torch.argsort(lab[keep], stable=True)]
+    # divided by a device tensor: torch multiplies by the reciprocal of a Python scalar, which is not s / fs to the bit
+    T = sd[rows].double() / torch.tensor(float(fs), dtype=torch.float64, device=dev)
+    pos = _dev(cable_pos, dev)[ch[rows]]
+    off = torch.zeros(K + 1, dtype=torch.int64, device=dev)
+    off[1:] = torch.cumsum(res.count, 0)
+    nx, ny = len(axes[0]), len(axes[1])
+    gx, gy, gz = (_dev(a, dev) for a in axes)
+    g = res.node
+    n0 = torch.stack([gx[g % nx], gy[(g // nx) % ny], gz[g // (nx * ny)], res.t0], 1)
+    return T.contiguous(), pos.contiguous(), off, n0
 
 
 # ------------------------------------------------------------------------------ reference signatures on the GPU
