@@ -2,6 +2,7 @@
 // translation units of libd4w.so.
 #pragma once
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <atomic>
 #include <string>
 #include <vector>
@@ -47,5 +48,19 @@ struct DeviceGuard {
     explicit DeviceGuard(int dev) { cudaGetDevice(&prev); if (prev != dev) cudaSetDevice(dev); else prev = -1; }
     ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
+
+// Rows per launch of the row kernels, which put one row (or row pair) on each blockIdx.y: gridDim.y <= 65 535.
+constexpr int kMaxGridRows = 65535;
+
+// launch(r0, rows) for consecutive blocks of at most `block` rows covering [0, nrows), until one returns an error.  r0 is a
+// size_t so that the caller's pointer offsets (r0 * row length) are computed in size_t.
+template <class F>
+inline int for_row_blocks(int nrows, int block, F&& launch) {
+    for (int r0 = 0, rows = 0; r0 < nrows; r0 += rows) {
+        rows = std::min(block, nrows - r0);
+        if (const int rc = launch((size_t)r0, rows)) return rc;
+    }
+    return D4W_OK;
+}
 
 }  // namespace d4w

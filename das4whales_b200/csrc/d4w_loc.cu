@@ -66,17 +66,16 @@ extern "C" int d4w_loc_grid(const double* T, const double* pos, const long long*
     const size_t smem = loc_grid_smem_bytes(kLocGridThreads);
     D4W_CUDA_TRY(cudaFuncSetAttribute(k_loc_grid, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     LocBest* w = static_cast<LocBest*>(ws);
-    for (int c = 0; c < ncalls; c += 65535) {             // grid.y holds at most 65 535 calls per launch
-        const int m = ncalls - c < 65535 ? ncalls - c : 65535;
+    return for_row_blocks(ncalls, kMaxGridRows, [&](size_t c, int m) -> int {         // one call per blockIdx.y
         LocGridParams gc = g;
         gc.off = offsets + c;
-        LocBest* wc = w + (size_t)c * g.ntiles;
+        LocBest* wc = w + c * g.ntiles;
         k_loc_grid<<<dim3((unsigned)g.ntiles, (unsigned)m), kLocGridThreads, smem, st>>>(gc, wc);
         D4W_CHECK_LAUNCH("k_loc_grid");
-        k_loc_pick<<<(unsigned)m, kLocPickThreads, 0, st>>>(gc, wc, index + c, score + c, n0 + 4 * (size_t)c);
+        k_loc_pick<<<(unsigned)m, kLocPickThreads, 0, st>>>(gc, wc, index + c, score + c, n0 + 4 * c);
         D4W_CHECK_LAUNCH("k_loc_pick");
-    }
-    return D4W_OK;
+        return D4W_OK;
+    });
 }
 
 extern "C" int d4w_loc_solve(const double* T, const double* pos, const long long* offsets, int ncalls, double c0, int nbiter,

@@ -31,8 +31,6 @@ k_env_pack(const double* __restrict__ stx, const double* __restrict__ ste, const
     o[4] = var;
 }
 
-constexpr int kEnvMaxRows = 65535;          // rows per pass (d4w_hilbert's split rows take at most 65535)
-
 size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 // workspace for `rows` rows: [window copy if strided][envelope][Hilbert workspace][stats of x][stats of env][median]
@@ -53,7 +51,7 @@ EnvWs env_ws_layout(const d4w_row_plan* p, int rows, bool strided) {
 
 extern "C" size_t d4w_env_stats_workspace_bytes(const d4w_row_plan* p, int nrows, size_t ld) {
     if (!p || nrows < 1) return 0;
-    return env_ws_layout(p, std::min(nrows, kEnvMaxRows), ld != (size_t)p->ns).total;
+    return env_ws_layout(p, std::min(nrows, kMaxGridRows), ld != (size_t)p->ns).total;
 }
 
 extern "C" int d4w_env_stats(d4w_row_plan* p, const float* x, int nrows, size_t ld, double* out, void* ws, void* stream_v) {
@@ -63,15 +61,15 @@ extern "C" int d4w_env_stats(d4w_row_plan* p, const float* x, int nrows, size_t 
     DeviceGuard guard(p->device);
     cudaStream_t stream = (cudaStream_t)stream_v;
     const bool strided = ld != (size_t)n;
-    const EnvWs w = env_ws_layout(p, std::min(nrows, kEnvMaxRows), strided);
+    // passes of kMaxGridRows rows bound the workspace
+    const EnvWs w = env_ws_layout(p, std::min(nrows, kMaxGridRows), strided);
     char* base = static_cast<char*>(ws);
     float* env = reinterpret_cast<float*>(base + w.env);
     double* stx = reinterpret_cast<double*>(base + w.stx);
     double* ste = reinterpret_cast<double*>(base + w.ste);
     float* med = reinterpret_cast<float*>(base + w.med);
-    for (int r0 = 0; r0 < nrows; r0 += kEnvMaxRows) {
-        const int rows = std::min(kEnvMaxRows, nrows - r0);
-        const float* xr = x + (size_t)r0 * ld;
+    return for_row_blocks(nrows, kMaxGridRows, [&](size_t r0, int rows) -> int {
+        const float* xr = x + r0 * ld;
         if (strided) {
             float* xc = reinterpret_cast<float*>(base);
             D4W_CUDA_TRY(cudaMemcpy2DAsync(xc, (size_t)n * sizeof(float), xr, ld * sizeof(float), (size_t)n * sizeof(float), rows,
@@ -83,8 +81,8 @@ extern "C" int d4w_env_stats(d4w_row_plan* p, const float* x, int nrows, size_t 
         if (rc == D4W_OK) rc = d4w_row_stats(env, rows, n, 0, ste, nullptr, stream);
         if (rc == D4W_OK) rc = d4w_row_median_ld(env, rows, (size_t)n, (size_t)n, med, stream);
         if (rc != D4W_OK) return rc;
-        k_env_pack<<<(rows + 255) / 256, 256, 0, stream>>>(stx, ste, med, rows, out + 5 * (size_t)r0);
+        k_env_pack<<<(rows + 255) / 256, 256, 0, stream>>>(stx, ste, med, rows, out + 5 * r0);
         D4W_CHECK_LAUNCH("k_env_pack");
-    }
-    return D4W_OK;
+        return D4W_OK;
+    });
 }

@@ -208,8 +208,8 @@ extern "C" int d4w_row_plan_destroy(d4w_row_plan* p) {
 
 extern "C" size_t d4w_row_workspace_bytes(const d4w_row_plan* p, int nx) {
     if (!p || p->t1 == 1) return 16;
-    // two real rows share one complex workspace row
-    return (size_t)(nx + 1) / 2 * (size_t)(p->czt_m ? p->czt_m : p->ns) * sizeof(float2);
+    // two real rows share one complex workspace row; d4w_hilbert reuses it for each block of 2 * kMaxGridRows rows
+    return (size_t)(std::min(nx, 2 * kMaxGridRows) + 1) / 2 * (size_t)(p->czt_m ? p->czt_m : p->ns) * sizeof(float2);
 }
 
 extern "C" int d4w_row_plan_info(const d4w_row_plan* p, int* t1, int* t2, int* czt_m) {
@@ -256,14 +256,9 @@ static int hilbert_czt(d4w_row_plan* p, const float* x, float* out, int nx, void
     return rc == D4W_ERR_UNSUPPORTED ? fail(rc, "row split radix not built") : rc;
 }
 
-extern "C" int d4w_hilbert(d4w_row_plan* p, const float* x, float* out, int nx, void* workspace, int mode,
-                           const double* dev_stats, void* stream_v) {
-    if (!p || !x || !out || nx < 1) return fail(D4W_ERR_ARG, "d4w_hilbert: bad argument");
-    if (mode < 0 || mode > EPI_ENVSTD) return fail(D4W_ERR_ARG, "d4w_hilbert: mode must be 0..3");
-    if ((mode == EPI_SNR || mode == EPI_ENVSTD) && !dev_stats) return fail(D4W_ERR_ARG, "d4w_hilbert: this mode needs row statistics");
-    if (nx > 65535 && p->t1 > 1) return fail(D4W_ERR_UNSUPPORTED, "d4w_hilbert: more than 65535 rows per call");
-    DeviceGuard guard(p->device);
-    cudaStream_t stream = (cudaStream_t)stream_v;
+// nx rows in one launch per kernel
+static int hilbert_rows(d4w_row_plan* p, const float* x, float* out, int nx, void* workspace, int mode, const double* dev_stats,
+                        cudaStream_t stream) {
     if (p->czt_m) return hilbert_czt(p, x, out, nx, workspace, mode, dev_stats, stream);
     if (p->t1 == 1) {
         k_hilbert_row<<<nx, 256, p->row_smem, stream>>>(p->row, x, out, p->d_hilbert, mode, dev_stats);
@@ -291,6 +286,21 @@ extern "C" int d4w_hilbert(d4w_row_plan* p, const float* x, float* out, int nx, 
         return D4W_OK;
     });
     return rc == D4W_ERR_UNSUPPORTED ? fail(rc, "row split radix not built") : rc;
+}
+
+extern "C" int d4w_hilbert(d4w_row_plan* p, const float* x, float* out, int nx, void* workspace, int mode,
+                           const double* dev_stats, void* stream_v) {
+    if (!p || !x || !out || nx < 1) return fail(D4W_ERR_ARG, "d4w_hilbert: bad argument");
+    if (mode < 0 || mode > EPI_ENVSTD) return fail(D4W_ERR_ARG, "d4w_hilbert: mode must be 0..3");
+    if ((mode == EPI_SNR || mode == EPI_ENVSTD) && !dev_stats) return fail(D4W_ERR_ARG, "d4w_hilbert: this mode needs row statistics");
+    DeviceGuard guard(p->device);
+    // Split rows take at most kMaxGridRows row pairs per launch.  Their blocks start on even rows, so every row keeps the
+    // partner it has in a call on its block alone; whole rows (one CTA per row on blockIdx.x) go in one launch.
+    const int block = p->t1 > 1 ? 2 * kMaxGridRows : nx;
+    return for_row_blocks(nx, block, [&](size_t r0, int rows) -> int {
+        return hilbert_rows(p, x + r0 * p->ns, out + r0 * p->ns, rows, workspace, mode, dev_stats ? dev_stats + 4 * r0 : nullptr,
+                            (cudaStream_t)stream_v);
+    });
 }
 
 // ------------------------------------------------------------------ forward-backward SOS IIR
@@ -362,7 +372,6 @@ extern "C" int d4w_stft_mag(d4w_fft_plan* p, const float* x, float* out, int nx,
                             int bin_lo, int bin_hi, void* stream_v) {
     if (!p || !x || !out || !dev_window) return fail(D4W_ERR_ARG, "d4w_stft_mag: null argument");
     if (p->n % 2 || hop < 1) return fail(D4W_ERR_ARG, "d4w_stft_mag: n_fft must be even and hop >= 1");
-    if (nx > 65535) return fail(D4W_ERR_UNSUPPORTED, "d4w_stft_mag: more than 65535 rows per call");
     DeviceGuard guard(p->device);
     StftParams sp{};
     sp.pl = p->pl; sp.tw = p->d_tw; sp.k2pos = p->d_k2pos;
@@ -374,10 +383,12 @@ extern "C" int d4w_stft_mag(d4w_fft_plan* p, const float* x, float* out, int nx,
     const size_t smem = (size_t)(fpb / 2) * (p->n + 1) * sizeof(float2);
     if (smem > p->smem_cap) return fail(D4W_ERR_UNSUPPORTED, "d4w_stft_mag: n_fft too large for shared memory");
     D4W_CUDA_TRY(cudaFuncSetAttribute(k_stft_mag, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cap));
-    dim3 grid((sp.nframes + fpb - 1) / fpb, nx);
-    k_stft_mag<<<grid, 256, smem, (cudaStream_t)stream_v>>>(sp, x, dev_window, out);
-    D4W_CHECK_LAUNCH("k_stft_mag");
-    return D4W_OK;
+    return for_row_blocks(nx, kMaxGridRows, [&](size_t r0, int rows) -> int {
+        dim3 grid((sp.nframes + fpb - 1) / fpb, rows);
+        k_stft_mag<<<grid, 256, smem, (cudaStream_t)stream_v>>>(sp, x + r0 * ns, dev_window, out + r0 * sp.nbins * sp.nframes);
+        D4W_CHECK_LAUNCH("k_stft_mag");
+        return D4W_OK;
+    });
 }
 
 // sliding-DFT variant for a band of bins of heavily overlapping Hann frames (k_stft_slide); n_fft = hop * P
@@ -392,10 +403,12 @@ static int launch_stft_slide_g(d4w_fft_plan* p, const float* x, float* out, int 
     if (smem > p->smem_cap) return fail(D4W_ERR_UNSUPPORTED, "d4w_stft_slide: tile does not fit shared memory");
     D4W_CUDA_TRY(cudaFuncSetAttribute(k_stft_slide<H, P, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cap));
     const int threads = std::min(kSlideMaxThreads, std::max((G * sp.nY + 31) / 32 * 32, 320));
-    dim3 grid((sp.nframes + G * R - 1) / (G * R), nx);
-    k_stft_slide<H, P, G><<<grid, threads, smem, st>>>(sp, x, p->d_wn, out);
-    D4W_CHECK_LAUNCH("k_stft_slide");
-    return D4W_OK;
+    return for_row_blocks(nx, kMaxGridRows, [&](size_t r0, int rows) -> int {
+        dim3 grid((sp.nframes + G * R - 1) / (G * R), rows);
+        k_stft_slide<H, P, G><<<grid, threads, smem, st>>>(sp, x + r0 * sp.ns, p->d_wn, out + r0 * sp.nbins * sp.nframes);
+        D4W_CHECK_LAUNCH("k_stft_slide");
+        return D4W_OK;
+    });
 }
 
 // runs per CTA: narrow bands take more runs so that runs x (bins + 2) threads fill the CTA
@@ -417,7 +430,6 @@ extern "C" int d4w_stft_slide(d4w_fft_plan* p, const float* x, float* out, int n
     if (!p || !x || !out) return fail(D4W_ERR_ARG, "d4w_stft_slide: null argument");
     if (bin_lo < 0 || bin_hi > p->n / 2 || bin_lo > bin_hi) return fail(D4W_ERR_ARG, "d4w_stft_slide: bad bin range");
     if (nx < 1 || ns < 1) return fail(D4W_ERR_ARG, "d4w_stft_slide: empty input");
-    if (nx > 65535) return fail(D4W_ERR_UNSUPPORTED, "d4w_stft_slide: more than 65535 rows per call");
     const int nbins = bin_hi - bin_lo + 1;
     if (!d4w_stft_slide_supported(p->n, hop, nbins) || !p->d_wn)
         return fail(D4W_ERR_UNSUPPORTED, "d4w_stft_slide: (n_fft, hop, band) not covered, use d4w_stft_mag");
@@ -529,7 +541,7 @@ static int launch_speccorr_untiled(const float* S, int nx, int nfs, int nt, cons
 }
 
 // All kernels in one k_speccorr4 pass when their tile fits; otherwise one pass per kernel, tiled or untiled.
-static int speccorr_kernels(const float* S, int nx, int nfs, int nt, const SpecKernel* ks, int nk, cudaStream_t st) {
+static int speccorr_block(const float* S, int nx, int nfs, int nt, const SpecKernel* ks, int nk, cudaStream_t st) {
     SpecCorrSet set;
     size_t smem = speccorr4_set(ks, nk, nfs, set);
     if (smem <= 110 * 1024) return launch_speccorr4(S, nx, nt, set, smem, st);
@@ -542,10 +554,21 @@ static int speccorr_kernels(const float* S, int nx, int nfs, int nt, const SpecK
     return D4W_OK;
 }
 
+static int speccorr_kernels(const float* S, int nx, int nfs, int nt, const SpecKernel* ks, int nk, cudaStream_t st) {
+    return for_row_blocks(nx, kMaxGridRows, [&](size_t r0, int rows) -> int {
+        SpecKernel kb[kScMaxKernels];
+        for (int k = 0; k < nk; ++k) {
+            kb[k] = ks[k];
+            kb[k].med += r0;
+            kb[k].out += r0 * nt;
+        }
+        return speccorr_block(S + r0 * nfs * nt, rows, nfs, nt, kb, nk, st);
+    });
+}
+
 extern "C" int d4w_speccorr(const float* S, int nx, int nf, int nt, const float* K, int kw, const float* med, float* out,
                             void* stream) {
     if (!S || !K || !med || !out || nx < 1 || nf < 1 || nt < 1 || kw < 1) return fail(D4W_ERR_ARG, "d4w_speccorr: bad argument");
-    if (nx > 65535) return fail(D4W_ERR_UNSUPPORTED, "d4w_speccorr: more than 65535 rows per call");
     const SpecKernel kk{K, med, out, 0, nf, kw};
     return speccorr_kernels(S, nx, nf, nt, &kk, 1, (cudaStream_t)stream);
 }
@@ -561,39 +584,41 @@ extern "C" int d4w_speccorr_multi(const float* S, int nx, int nf, int nt, int nk
             return fail(D4W_ERR_ARG, "d4w_speccorr_multi: bad kernel");
         ks[k] = SpecKernel{K[k], med[k], out[k], f0[k], nfk[k], kw[k]};
     }
-    if (nx > 65535) return fail(D4W_ERR_UNSUPPORTED, "d4w_speccorr_multi: more than 65535 rows per call");
     return speccorr_kernels(S, nx, nf, nt, ks, nk, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------- peak picking
 static void peak_level_sizes(int ns, int& nb1, int& nb2) { nb1 = (ns + kPkB - 1) / kPkB; nb2 = (nb1 + kPkB - 1) / kPkB; }
 
+// the workspace holds one block of rows, reused by the next in stream order
 extern "C" size_t d4w_find_peaks_workspace_bytes(int nx, int ns) {
     if (nx < 1 || ns < 1) return 0;
     int nb1, nb2; peak_level_sizes(ns, nb1, nb2);
-    return ((size_t)nx * (2 * (size_t)nb1 + 2 * (size_t)nb2 + 1)) * sizeof(float) + 256;
+    return ((size_t)std::min(nx, kMaxGridRows) * (2 * (size_t)nb1 + 2 * (size_t)nb2 + 1)) * sizeof(float) + 256;
 }
 
 extern "C" int d4w_find_peaks(const float* x, int nx, int ns, double prominence, unsigned char* flags, void* ws, void* stream_v) {
     if (!x || !flags || !ws || nx < 1 || ns < 1) return fail(D4W_ERR_ARG, "d4w_find_peaks: bad argument");
-    if (nx > 65535) return fail(D4W_ERR_UNSUPPORTED, "d4w_find_peaks: more than 65535 rows per call");
     if (!(prominence >= 0.0)) return fail(D4W_ERR_ARG, "d4w_find_peaks: prominence must be >= 0");
     cudaStream_t stream = (cudaStream_t)stream_v;
     D4W_CUDA_TRY(cudaMemsetAsync(flags, 0, (size_t)nx * ns, stream));
     if (ns < 3) return D4W_OK;
     int nb1, nb2; peak_level_sizes(ns, nb1, nb2);
-    float* bmax = reinterpret_cast<float*>(ws);
-    float* bmin = bmax + (size_t)nx * nb1;
-    float* smax = bmin + (size_t)nx * nb1;
-    float* smin = smax + (size_t)nx * nb2;
-    float* rowmin = smin + (size_t)nx * nb2;
-    k_peak_levels<<<nx, 256, 0, stream>>>(x, ns, bmax, bmin, smax, smin, rowmin, nb1, nb2);
-    D4W_CHECK_LAUNCH("k_peak_levels");
-    PeakLevels lv{bmax, bmin, smax, smin, nb1, nb2};
-    dim3 grid((ns + 255) / 256, nx);
-    k_peak_pick<<<grid, 256, 0, stream>>>(x, ns, lv, rowmin, prominence, flags);
-    D4W_CHECK_LAUNCH("k_peak_pick");
-    return D4W_OK;
+    return for_row_blocks(nx, kMaxGridRows, [&](size_t r0, int rows) -> int {
+        float* bmax = reinterpret_cast<float*>(ws);
+        float* bmin = bmax + (size_t)rows * nb1;
+        float* smax = bmin + (size_t)rows * nb1;
+        float* smin = smax + (size_t)rows * nb2;
+        float* rowmin = smin + (size_t)rows * nb2;
+        const float* xb = x + r0 * ns;
+        k_peak_levels<<<rows, 256, 0, stream>>>(xb, ns, bmax, bmin, smax, smin, rowmin, nb1, nb2);
+        D4W_CHECK_LAUNCH("k_peak_levels");
+        PeakLevels lv{bmax, bmin, smax, smin, nb1, nb2};
+        dim3 grid((ns + 255) / 256, rows);
+        k_peak_pick<<<grid, 256, 0, stream>>>(xb, ns, lv, rowmin, prominence, flags + r0 * ns);
+        D4W_CHECK_LAUNCH("k_peak_pick");
+        return D4W_OK;
+    });
 }
 
 // ---------------------------------------------------------------------------------- raw counts -> strain

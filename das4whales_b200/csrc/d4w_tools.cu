@@ -141,9 +141,10 @@ extern "C" int d4w_row_moments(const float* x, size_t ld, int nrows, int n, int 
 extern "C" int d4w_detrend_linear(const float* x, size_t ld, int nrows, int n, const double* mom, float* y, void* stream_v) {
     if (!x || !mom || !y) return fail(D4W_ERR_ARG, "d4w_detrend_linear: null pointer");
     if (nrows < 1 || n < 1 || ld < (size_t)n) return fail(D4W_ERR_ARG, "d4w_detrend_linear: need nrows, n >= 1 and ld >= n");
-    if (nrows > 65535) return fail(D4W_ERR_UNSUPPORTED, "d4w_detrend_linear: more than 65 535 rows in one call");
-    const dim3 grid((unsigned)std::min((n + 255) / 256, 64), (unsigned)nrows);
-    k_detrend<<<grid, 256, 0, (cudaStream_t)stream_v>>>(x, ld, nrows, n, mom, y);
-    D4W_CHECK_LAUNCH("k_detrend");
-    return D4W_OK;
+    return for_row_blocks(nrows, kMaxGridRows, [&](size_t r0, int rows) -> int {
+        const dim3 grid((unsigned)std::min((n + 255) / 256, 64), (unsigned)rows);
+        k_detrend<<<grid, 256, 0, (cudaStream_t)stream_v>>>(x + r0 * ld, ld, rows, n, mom + r0 * 3, y + r0 * n);
+        D4W_CHECK_LAUNCH("k_detrend");
+        return D4W_OK;
+    });
 }

@@ -25,12 +25,12 @@ struct d4w_fft_plan {
 namespace d4w {
 
 // One dispatch for both modes (rows_kernels.cuh, k_xcorr*): SAME = false is d4w_xcorr, SAME = true d4w_xcorr_same.
+// nx rows of one launch; out_tpl_stride is the distance between the templates' output matrices.
 template <bool SAME>
-static int xcorr_launch(d4w_fft_plan* p, const float* x, int nx, int ns, int valid, int ntpl, const void* dev_tabs,
-                        const double* dev_mu_over_m, const double* dev_stats, const double* dev_segpre, const float* dev_rowmax,
-                        int lag0, float* out, void* stream) {
+static int xcorr_launch_block(d4w_fft_plan* p, const float* x, int nx, int ns, int valid, int ntpl, const void* dev_tabs,
+                              const double* dev_mu_over_m, const double* dev_stats, const double* dev_segpre,
+                              const float* dev_rowmax, int lag0, float* out, size_t out_tpl_stride, void* stream) {
     const char* fn = SAME ? "d4w_xcorr_same" : "d4w_xcorr";
-    DeviceGuard guard(p->device);
     XcorrParams xp{};
     xp.pl = p->pl; xp.tw = p->d_tw; xp.nb = p->n; xp.valid = valid; xp.ntpl = ntpl; xp.ns = ns;
     xp.normalize = dev_stats != nullptr ? 1 : 0;
@@ -44,7 +44,7 @@ static int xcorr_launch(d4w_fft_plan* p, const float* x, int nx, int ns, int val
         if (smem_pfa > 112 * 1024) return fail(D4W_ERR_UNSUPPORTED, std::string(fn) + ": shared memory");
         dim3 gridp((xp.nseg + 3) / 4, nx);
         k_xcorr_pfa<SAME><<<gridp, kPfaThreads, smem_pfa, (cudaStream_t)stream>>>(xp, p->d_tpos, x, (const float2*)dev_tabs, dev_stats,
-                                                                          dev_segpre, dev_mu_over_m, out, (size_t)nx * ns,
+                                                                          dev_segpre, dev_mu_over_m, out, out_tpl_stride,
                                                                           dev_rowmax, lag0);
         D4W_CHECK_LAUNCH("k_xcorr_pfa");
         return D4W_OK;
@@ -55,7 +55,7 @@ static int xcorr_launch(d4w_fft_plan* p, const float* x, int nx, int ns, int val
         D4W_CUDA_TRY(cudaFuncSetAttribute(k_xcorr_dual<SAME>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
         dim3 gridd((xp.nseg + 3) / 4, nx);
         k_xcorr_dual<SAME><<<gridd, 256, smem_dual, (cudaStream_t)stream>>>(xp, x, (const float2*)dev_tabs, dev_stats, dev_segpre,
-                                                                           dev_mu_over_m, out, (size_t)nx * ns, dev_rowmax, lag0);
+                                                                           dev_mu_over_m, out, out_tpl_stride, dev_rowmax, lag0);
         D4W_CHECK_LAUNCH("k_xcorr_dual");
         return D4W_OK;
     }
@@ -65,14 +65,28 @@ static int xcorr_launch(d4w_fft_plan* p, const float* x, int nx, int ns, int val
     if (p->fused) {
         D4W_CUDA_TRY(cudaFuncSetAttribute(k_xcorr_fused<SAME>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cap - 1024));
         k_xcorr_fused<SAME><<<grid, 128, smem, (cudaStream_t)stream>>>(xp, x, (const float2*)dev_tabs, dev_stats, dev_segpre, dev_mu_over_m,
-                                                                      out, (size_t)nx * ns, dev_rowmax, lag0);
+                                                                      out, out_tpl_stride, dev_rowmax, lag0);
     } else {
         D4W_CUDA_TRY(cudaFuncSetAttribute(k_xcorr<SAME>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cap - 1024));  // minus its static smem
         k_xcorr<SAME><<<grid, 128, smem, (cudaStream_t)stream>>>(xp, x, (const float2*)dev_tabs, dev_stats, dev_segpre, dev_mu_over_m, out,
-                                                                (size_t)nx * ns, dev_rowmax, lag0);
+                                                                out_tpl_stride, dev_rowmax, lag0);
     }
     D4W_CHECK_LAUNCH("k_xcorr");
     return D4W_OK;
+}
+
+// Any number of rows, in blocks of kMaxGridRows; out is [ntpl][nx][ns] for the whole call.
+template <bool SAME>
+static int xcorr_launch(d4w_fft_plan* p, const float* x, int nx, int ns, int valid, int ntpl, const void* dev_tabs,
+                        const double* dev_mu_over_m, const double* dev_stats, const double* dev_segpre, const float* dev_rowmax,
+                        int lag0, float* out, void* stream) {
+    DeviceGuard guard(p->device);
+    const int nseg = (ns + valid - 1) / valid;
+    return for_row_blocks(nx, kMaxGridRows, [&](size_t r0, int rows) -> int {
+        return xcorr_launch_block<SAME>(p, x + r0 * ns, rows, ns, valid, ntpl, dev_tabs, dev_mu_over_m,
+                                        dev_stats ? dev_stats + 4 * r0 : nullptr, dev_segpre ? dev_segpre + r0 * nseg : nullptr,
+                                        dev_rowmax ? dev_rowmax + r0 : nullptr, lag0, out + r0 * ns, (size_t)nx * ns, stream);
+    });
 }
 
 }  // namespace d4w

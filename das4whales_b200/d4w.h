@@ -197,7 +197,7 @@ int d4w_snr(const float* dev_x, float* dev_out, int nx, int ns, const double* de
  *      overlap-save FFT correlation; `plan` = fft plan of the block length nb, `valid` = nb - L + 1
  *      lags kept per block.  dev_tabs: ntpl x nb complex64 = conj(FFT_nb(template_t)) / (nb * m_t) in
  *      the plan's table order (d4w_fft_plan_table_order).  With dev_stats != NULL rows are demeaned / peak-normalised and
- *      the mean-of-padded-template term mu_t/m_t * prefix is added (dev_mu_over_m: double[ntpl]).
+ *      the mean-of-padded-template term mu_t/m_t * prefix is added (dev_mu_over_m: double[ntpl]).  Any number of rows.
  *      dev_out: float32 [ntpl][nx][ns]. */
 int d4w_xcorr(d4w_fft_plan* plan, const float* dev_x, int nx, int ns, int valid, int ntpl, const void* dev_tabs,
               const double* dev_mu_over_m, const double* dev_stats, const double* dev_segpre, float* dev_out,
@@ -207,7 +207,7 @@ int d4w_xcorr(d4w_fft_plan* plan, const float* dev_x, int nx, int ns, int valid,
  *      out[t][row][i] = sum_n x[row][i - lag0 + n] c'_t[n] / rowmax[row], x = 0 outside [0, ns), where c'_t is template t with
  *      lag0 - floor(L_t / 2) zeros prepended (lag0 = max_t floor(L_t / 2)).  dev_tabs: ntpl x nb complex64 =
  *      conj(FFT_nb(c'_t)) / nb in d4w_fft_plan_table_order; valid = nb - max_t len(c'_t) + 1.  dev_rowmax: float[nx] from
- *      d4w_row_max (clamped at 0); rows with !(rowmax > 0) are written as zeros.  1 <= nx <= 65535.
+ *      d4w_row_max (clamped at 0); rows with !(rowmax > 0) are written as zeros.  Any nx >= 1.
  *      dev_out: float32 [ntpl][nx][ns]. */
 int d4w_xcorr_same(d4w_fft_plan* plan, const float* dev_x, int nx, int ns, int valid, int lag0, int ntpl, const void* dev_tabs,
                    const float* dev_rowmax, float* dev_out, void* stream);
@@ -218,7 +218,9 @@ int d4w_xcorr_same(d4w_fft_plan* plan, const float* dev_x, int nx, int ns, int v
  *      d4w_xcorr's dev_tabs are in d4w_fft_plan_table_order.
  *      Any ns up to 128 000 is accepted: a length with no T1 x T2 split (a prime factor > 61) is transformed by a chirp-z
  *      convolution of length czt_m = T1 * T2 ~ 2 ns.  d4w_row_plan_info reports the split and czt_m (0: direct transform);
- *      d4w_row_workspace_bytes sizes the workspace for nx rows of the chosen route. */
+ *      d4w_row_workspace_bytes sizes the workspace for nx rows of the chosen route.  Any number of rows: split rows go in
+ *      blocks of 2 x 65 535 that reuse one block's workspace in stream order, so the bytes for min(nx, 131 070) rows
+ *      suffice (a larger workspace is fine). */
 int d4w_row_plan_create(d4w_row_plan** out, int ns, int device);
 int d4w_row_plan_destroy(d4w_row_plan* plan);
 size_t d4w_row_workspace_bytes(const d4w_row_plan* plan, int nx);
@@ -229,8 +231,8 @@ int d4w_hilbert(d4w_row_plan* plan, const float* dev_x, float* dev_out, int nx, 
  * dev_x + r * ld (ld >= n), n = the row plan's length (any n up to 128 000, as d4w_hilbert).  out: double[nrows][5] =
  * {median |hilbert(x)|, mean |hilbert(x)|, mean x, mean x^2, population variance of x}; a row of variance 0 is constant and
  * gets the envelope statistics |mean x| exactly (0 for a zero channel).
- * dev_workspace: d4w_env_stats_workspace_bytes(plan, nrows, ld) bytes (the envelope of up to 65 535 rows, and a dense copy of
- * the window when ld != n).  Any nrows >= 1. */
+ * dev_workspace: d4w_env_stats_workspace_bytes(plan, nrows, ld) bytes (the envelope of one block of at most 65 535 rows,
+ * reused by the next in stream order, and a dense copy of the window when ld != n).  Any nrows >= 1. */
 size_t d4w_env_stats_workspace_bytes(const d4w_row_plan* plan, int nrows, size_t ld);
 int d4w_env_stats(d4w_row_plan* plan, const float* dev_x, int nrows, size_t ld, double* dev_out, void* dev_workspace, void* stream);
 
@@ -244,7 +246,7 @@ int d4w_sosfiltfilt(const float* dev_x, float* dev_y, float* dev_tmp, int nx, in
 /* ---- batched STFT magnitude with librosa.stft framing (dsp.get_spectrogram dsp.py:66-68,
  *      detect.get_sliced_nspectrogram detect.py:382): centred frames, zero padding, window
  *      dev_window[n_fft]; only DFT bins bin_lo..bin_hi (inclusive) are written (the band slice of
- *      detect.py:390-392): dev_out: float32 [nx][bin_hi-bin_lo+1][1 + ns/hop]. */
+ *      detect.py:390-392): dev_out: float32 [nx][bin_hi-bin_lo+1][1 + ns/hop].  Any number of rows. */
 int d4w_stft_mag(d4w_fft_plan* plan, const float* dev_x, float* dev_out, int nx, int ns, int hop,
                  const float* dev_window, int bin_lo, int bin_hi, void* stream);
 
@@ -252,7 +254,7 @@ int d4w_stft_mag(d4w_fft_plan* plan, const float* dev_x, float* dev_out, int nx,
  * (n_fft = hop * P): sliding DFT, every sample enters one block sum per bin instead of one FFT per frame.  Shapes covered:
  * d4w_stft_slide_supported(n_fft, hop, bin_hi - bin_lo + 1) != 0; anything else returns D4W_ERR_UNSUPPORTED.
  * Replaces the librosa.stft call of detect.get_sliced_nspectrogram inside the channel loop of
- * detect.compute_cross_correlogram_spectrocorr (/root/reference/src/das4whales/detect.py:334-408, :700-707). */
+ * detect.compute_cross_correlogram_spectrocorr (/root/reference/src/das4whales/detect.py:334-408, :700-707).  Any nx >= 1. */
 int d4w_stft_slide_supported(int nfft, int hop, int nbins);
 int d4w_stft_slide(d4w_fft_plan* plan, const float* x, float* out, int nx, int ns, int hop, int bin_lo, int bin_hi,
                    void* stream);
@@ -300,7 +302,8 @@ int d4w_csd(d4w_fft_plan* plan, const float* dev_x, long long x_row_stride, cons
 /* ---- spectrogram-correlation detector: detect.xcorr2d / compute_cross_correlogram_spectrocorr
  *      (detect.py:579-602, :650-708).  Per-row median / maximum of a float32 matrix [nrows][n]
  *      (entries must be >= 0 for the median), and
- *      out[row][t] = max(0, sum_f sum_j S[row][f][t - kw/2 + j] K[f][j]) / (med[row] * kw). */
+ *      out[row][t] = max(0, sum_f sum_j S[row][f][t - kw/2 + j] K[f][j]) / (med[row] * kw).  d4w_speccorr and
+ *      d4w_speccorr_multi take any nx >= 1. */
 int d4w_row_median(const float* dev_x, int nrows, size_t n, float* dev_median, void* stream);
 int d4w_row_max(const float* dev_x, int nrows, size_t n, float* dev_max, void* stream);
 int d4w_speccorr(const float* dev_S, int nx, int nf, int nt, const float* dev_K, int kw, const float* dev_median,
@@ -318,7 +321,8 @@ int d4w_speccorr_multi(const float* dev_S, int nx, int nf, int nt, int nk, const
  *      (:249-274, :271): scipy.signal.find_peaks(row, prominence=threshold) on every row of a [nx][ns] float32 matrix
  *      (flat tops -> plateau midpoint, prominence walked to the nearest strictly greater sample, compared in double).
  *      flags[nx][ns] (bytes) is cleared and set to 1 at every accepted peak; ws needs
- *      d4w_find_peaks_workspace_bytes(nx, ns) bytes. */
+ *      d4w_find_peaks_workspace_bytes(nx, ns) bytes.  Any nx >= 1: rows go in blocks of 65 535 that reuse one block's
+ *      workspace in stream order, so the bytes for min(nx, 65 535) rows suffice (a larger workspace is fine). */
 size_t d4w_find_peaks_workspace_bytes(int nx, int ns);
 int d4w_find_peaks(const float* dev_x, int nx, int ns, double prominence, unsigned char* dev_flags, void* dev_ws, void* stream);
 
@@ -428,7 +432,7 @@ int d4w_grad_oriented(const float* dev_in, int h, int w, int dft, int dfx, float
  *      dev_x + r * ld, chunk c its samples [c chunk, min((c + 1) chunk, n)), t counted from the chunk start.
  *      dev_out: double [nrows][ceil(n / chunk)][3].
  *  d4w_detrend_linear: scipy.signal.detrend(type='linear', axis=-1) of the same rows (moments of chunk = n from
- *      d4w_row_moments), written contiguously: dev_y float32 [nrows][n].  nrows <= 65 535. */
+ *      d4w_row_moments), written contiguously: dev_y float32 [nrows][n].  Any nrows >= 1. */
 size_t d4w_fan_blur_workspace_bytes(int nx, double sigma);
 int d4w_fan_blur(float* dev_out, int nx, int ns, double kval, double fval, double c_min, double c_max, double sigma,
                  void* dev_workspace, void* stream);

@@ -95,14 +95,14 @@ def compute_cross_correlogram(data, template):
     rows demeaned and divided by their raw abs-max, template (zero-padded to ns) demeaned and
     divided by its abs-max, positive lags of the full correlation."""
     xd = _to_device(data)
-    out = _rows.cross_correlogram_chunked(xd, [np.asarray(template, dtype=np.float64)], normalize=True)[0]
+    out = _rows.cross_correlogram(xd, [np.asarray(template, dtype=np.float64)], normalize=True)[0]
     return out if _is_tensor(data) else _to_host64(out)
 
 
 def compute_cross_correlograms(data, templates):
     """Several templates in ONE pass over the data (HF + LF notes of scripts/main_mfdetect.py:79-80)."""
     xd = _to_device(data)
-    outs = _rows.cross_correlogram_chunked(xd, [np.asarray(t, dtype=np.float64) for t in templates], normalize=True)
+    outs = _rows.cross_correlogram(xd, [np.asarray(t, dtype=np.float64) for t in templates], normalize=True)
     return outs if _is_tensor(data) else [_to_host64(o) for o in outs]
 
 
@@ -311,7 +311,7 @@ def _spectrocorr_device(xd, nperseg, nhop, union, per_kernel):
     b0, b1 = union
     nf, nt = b1 - b0 + 1, 1 + ns // nhop
     outs = [torch.empty((nx, nt), dtype=torch.float32, device=xd.device) for _ in per_kernel]
-    chunk = max(1, min(nx, _rows._MAX_ROWS, (2 << 30) // max(1, nf * nt * 4)))
+    chunk = max(1, min(nx, (2 << 30) // max(1, nf * nt * 4)))
     for r0 in range(0, nx, chunk):
         S = _rows.stft_mag(xd[r0:r0 + chunk], nperseg, nhop, b0, b1)
         n = S.shape[0]

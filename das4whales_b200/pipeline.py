@@ -171,7 +171,7 @@ class MfDetectPipeline(_FilePipeline):
         torch = self.torch
         with torch.cuda.device(self.device):
             y = self._filtered(raw)
-            corr = _rows.cross_correlogram_chunked(y, self.templates, normalize=True)
+            corr = _rows.cross_correlogram(y, self.templates, normalize=True)
             del y
             return self._pick(corr, with_snr)
 

@@ -112,7 +112,7 @@ def _pick_block(L, ns=0):
 
 def cross_correlogram(x, templates, normalize=True):
     """Positive-lag correlation of every row with each template (detect.py:96-166).
-    templates: list of 1-D float64 arrays (zero-padded to ns, as gen_template_fincall returns).
+    templates: list of 1-D float64 arrays (zero-padded to ns, as gen_template_fincall returns).  Any number of rows.
     Returns a list of float32 CUDA tensors [nx, ns]."""
     torch = _torch()
     dev = _check_input(x)
@@ -158,29 +158,6 @@ def cross_correlogram(x, templates, normalize=True):
     return [out[i] for i in range(len(taps))]
 
 
-_MAX_ROWS = 65535       # gridDim.y limit of the row kernels
-
-
-def _row_chunked(corr, x, ntpl):
-    """corr(rows) -> ntpl float32 tensors [len(rows), ns], for any number of rows: corr is called on slices of <= 65535 rows
-    (the kernels' launch limit) and the parts are copied into whole-matrix outputs."""
-    torch = _torch()
-    nx = x.shape[0]
-    if nx <= _MAX_ROWS:
-        return corr(slice(0, nx))
-    outs = [torch.empty_like(x) for _ in range(ntpl)]
-    for r0 in range(0, nx, _MAX_ROWS):
-        part = corr(slice(r0, r0 + _MAX_ROWS))
-        for o, p in zip(outs, part):
-            o[r0:r0 + _MAX_ROWS] = p
-    return outs
-
-
-def cross_correlogram_chunked(x, templates, normalize=True):
-    """cross_correlogram for any number of rows (the kernels take <= 65535 rows per launch)."""
-    return _row_chunked(lambda rs: cross_correlogram(x[rs], templates, normalize), x, len(templates))
-
-
 def same_mode_layout(templates, ns):
     """Host side of the "same"-mode correlation (d4w_xcorr_same), pure NumPy.
     templates: 1-D tap arrays c_t (un-padded, any lengths).  Template t gets D - floor(L_t / 2) zeros prepended, D = max_t
@@ -214,15 +191,11 @@ def cross_correlogram_same(x, templates):
     with torch.cuda.device(dev):
         tabs_d = torch.from_numpy(tabs.view(np.float32).reshape(ntpl, nb, 2)).to(x.device)
         rowmax = row_max(x)                                   # clamped at 0: "> 0" is the script's test, the value its max
-
-        def corr(rs):
-            xs = x[rs]
-            out = torch.empty((ntpl,) + tuple(xs.shape), dtype=torch.float32, device=x.device)
-            _lib.check(_lib.lib().d4w_xcorr_same(plan.ptr, _lib.ptr(xs, "float*"), xs.shape[0], ns, valid, lag0, ntpl,
-                                                 _lib.ptr(tabs_d), _lib.ptr(rowmax[rs], "float*"), _lib.ptr(out, "float*"),
-                                                 _lib.stream_ptr()), "xcorr_same")
-            return [out[i] for i in range(ntpl)]
-        return _row_chunked(corr, x, ntpl)
+        out = torch.empty((ntpl, nx, ns), dtype=torch.float32, device=x.device)
+        _lib.check(_lib.lib().d4w_xcorr_same(plan.ptr, _lib.ptr(x, "float*"), nx, ns, valid, lag0, ntpl, _lib.ptr(tabs_d),
+                                             _lib.ptr(rowmax, "float*"), _lib.ptr(out, "float*"), _lib.stream_ptr()),
+                   "xcorr_same")
+    return [out[i] for i in range(ntpl)]
 
 
 # ------------------------------------------------------------------------------ Hilbert envelope / SNR
@@ -234,9 +207,9 @@ def _hilbert(x, mode, stats=None):
     out = torch.empty_like(x)
     L = _lib.lib()
     with torch.cuda.device(dev):
-        # rows are independent: chunk so the complex workspace stays bounded (and gridDim.y <= 65535); a workspace row is
-        # ns complex samples on the direct route and czt_m ~ 2 ns on the chirp-z route
-        max_rows = max(1, min(65535, (8 << 30) // max(1, int(L.d4w_row_workspace_bytes(plan.ptr, 1)))))
+        # rows are independent: chunk so the complex workspace stays bounded; a workspace row is ns complex samples on the
+        # direct route and czt_m ~ 2 ns on the chirp-z route
+        max_rows = max(1, (8 << 30) // max(1, int(L.d4w_row_workspace_bytes(plan.ptr, 1))))
         wsb = L.d4w_row_workspace_bytes(plan.ptr, min(nx, max_rows))
         ws = torch.empty(int(wsb), dtype=torch.uint8, device=x.device)
         for r0 in range(0, nx, max_rows):
@@ -374,11 +347,11 @@ def stft_mag(x, nfft, hop, bin_lo=0, bin_hi=None):
         return _stft_frames(x, nfft, hop, bin_lo, bin_hi)
     plan = fft_plan(nfft, dev)
     out = torch.empty((nx, bin_hi - bin_lo + 1, 1 + ns // hop), dtype=torch.float32, device=x.device)
+    if nx == 0:
+        return out
     with torch.cuda.device(dev):
-        for r0 in range(0, nx, 65535):
-            r1 = min(nx, r0 + 65535)
-            _lib.check(L.d4w_stft_slide(plan.ptr, _lib.ptr(x[r0:r1], "float*"), _lib.ptr(out[r0:r1], "float*"), r1 - r0, ns,
-                                        int(hop), int(bin_lo), bin_hi, _lib.stream_ptr()), "stft_slide")
+        _lib.check(L.d4w_stft_slide(plan.ptr, _lib.ptr(x, "float*"), _lib.ptr(out, "float*"), nx, ns, int(hop), int(bin_lo),
+                                    bin_hi, _lib.stream_ptr()), "stft_slide")
     return out
 
 
@@ -394,11 +367,11 @@ def _stft_frames(x, nfft, hop, bin_lo, bin_hi):
         _tab_cache[key] = torch.from_numpy(sp.get_window("hann", nfft, fftbins=True).astype(np.float32)).to(x.device)
     win = _tab_cache[key]
     L = _lib.lib()
+    if nx == 0:
+        return out
     with torch.cuda.device(dev):
-        for r0 in range(0, nx, 65535):
-            r1 = min(nx, r0 + 65535)
-            _lib.check(L.d4w_stft_mag(plan.ptr, _lib.ptr(x[r0:r1], "float*"), _lib.ptr(out[r0:r1], "float*"), r1 - r0, ns,
-                                      int(hop), _lib.ptr(win, "float*"), int(bin_lo), bin_hi, _lib.stream_ptr()), "stft_mag")
+        _lib.check(L.d4w_stft_mag(plan.ptr, _lib.ptr(x, "float*"), _lib.ptr(out, "float*"), nx, ns, int(hop),
+                                  _lib.ptr(win, "float*"), int(bin_lo), bin_hi, _lib.stream_ptr()), "stft_mag")
     return out
 
 
@@ -551,6 +524,8 @@ def spectro_correlate_multi(S, kernels, offsets, medians, outs=None):
         outs = [torch.empty((nx, nt), dtype=torch.float32, device=S.device) for _ in Ks]
     if len(outs) != len(Ks) or any(o.dtype != torch.float32 or tuple(o.shape) != (nx, nt) or not o.is_contiguous() for o in outs):
         raise ValueError(f"outs must be contiguous float32 CUDA tensors [{nx}, {nt}]")
+    if nx == 0:
+        return outs
     ffi, L = _lib.ffi, _lib.lib()
     with torch.cuda.device(S.device.index):
         for g0 in range(0, len(Ks), SPECCORR_MAX_KERNELS):
@@ -559,12 +534,10 @@ def spectro_correlate_multi(S, kernels, offsets, medians, outs=None):
             nfk = ffi.new("int[]", [Ks[k].shape[0] for k in g])
             kw = ffi.new("int[]", [Ks[k].shape[1] for k in g])
             kp = ffi.new("float*[]", [_lib.ptr(Ks[k], "float*") for k in g])
-            for r0 in range(0, nx, _MAX_ROWS):
-                r1 = min(nx, r0 + _MAX_ROWS)
-                mp = ffi.new("float*[]", [_lib.ptr(medians[k][r0:r1], "float*") for k in g])
-                op = ffi.new("float*[]", [_lib.ptr(outs[k][r0:r1], "float*") for k in g])
-                _lib.check(L.d4w_speccorr_multi(_lib.ptr(S[r0:r1], "float*"), r1 - r0, nf, nt, len(g), f0, nfk, kp, kw, mp, op,
-                                                _lib.stream_ptr()), "speccorr_multi")
+            mp = ffi.new("float*[]", [_lib.ptr(medians[k], "float*") for k in g])
+            op = ffi.new("float*[]", [_lib.ptr(outs[k], "float*") for k in g])
+            _lib.check(L.d4w_speccorr_multi(_lib.ptr(S, "float*"), nx, nf, nt, len(g), f0, nfk, kp, kw, mp, op, _lib.stream_ptr()),
+                       "speccorr_multi")
     return outs
 
 
@@ -593,13 +566,13 @@ def find_peaks_flags(x2d, prominence):
     rows_, n = x2d.shape
     L = _lib.lib()
     flags = torch.empty((rows_, n), dtype=torch.uint8, device=x2d.device)
+    if rows_ == 0:
+        return flags
     with torch.cuda.device(x2d.device.index):
-        ws = torch.empty(int(L.d4w_find_peaks_workspace_bytes(min(rows_, 65535), n)), dtype=torch.uint8, device=x2d.device)
-        for r0 in range(0, rows_, 65535):
-            r1 = min(rows_, r0 + 65535)
-            _lib.check(L.d4w_find_peaks(_lib.ptr(x2d[r0:r1], "float*"), r1 - r0, n, float(prominence),
-                                        _lib.ffi.cast("unsigned char*", flags[r0:r1].data_ptr()), _lib.ptr(ws, "void*"),
-                                        _lib.stream_ptr()), "find_peaks")
+        ws = torch.empty(int(L.d4w_find_peaks_workspace_bytes(rows_, n)), dtype=torch.uint8, device=x2d.device)
+        _lib.check(L.d4w_find_peaks(_lib.ptr(x2d, "float*"), rows_, n, float(prominence),
+                                    _lib.ffi.cast("unsigned char*", flags.data_ptr()), _lib.ptr(ws, "void*"), _lib.stream_ptr()),
+                   "find_peaks")
     return flags
 
 
@@ -684,11 +657,8 @@ def detrend_linear(x, out=None):
     if out is None:
         out = torch.empty((rows_, n), dtype=torch.float32, device=x.device)
     with torch.cuda.device(dev):
-        for r0 in range(0, rows_, 65535):
-            r1 = min(rows_, r0 + 65535)
-            _lib.check(_lib.lib().d4w_detrend_linear(_lib.ptr(x[r0:r1], "float*"), max(x.stride(0), n), r1 - r0, n,
-                                                     _lib.ptr(mom[r0:r1], "double*"), _lib.ptr(out[r0:r1], "float*"),
-                                                     _lib.stream_ptr()), "detrend_linear")
+        _lib.check(_lib.lib().d4w_detrend_linear(_lib.ptr(x, "float*"), max(x.stride(0), n), rows_, n, _lib.ptr(mom, "double*"),
+                                                 _lib.ptr(out, "float*"), _lib.stream_ptr()), "detrend_linear")
     return out
 
 

@@ -43,7 +43,7 @@ def stages(xd, kernels, reps=REPS):
     nx, ns = xd.shape
     nperseg, nhop, _, (b0, b1), per = detect.spectrocorr_layout(FS, FLIMS, kernels, WIN, OV, ns)
     nf, nt = b1 - b0 + 1, 1 + ns // nhop
-    chunk = max(1, min(nx, rows._MAX_ROWS, (2 << 30) // max(1, nf * nt * 4)))
+    chunk = max(1, min(nx, (2 << 30) // max(1, nf * nt * 4)))
     outs = [torch.empty((nx, nt), dtype=torch.float32, device=xd.device) for _ in per]
     tot = np.zeros(3)
     for it in range(WARMUP + reps):
